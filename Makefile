@@ -20,16 +20,15 @@ bench: build
 	$(PY) bench.py
 
 sass:
-	cuobjdump -sass torchacc_b200/_C.so | grep -oE "UTC[A-Z0-9.]*MMA[A-Z0-9.]*|UTCCP[A-Z0-9.]*|UTMA[A-Z0-9.]*|UBLKCP[A-Z0-9.]*|LDTM[A-Z0-9.]*|STTM[A-Z0-9.]*|USETMAXREG[A-Z0-9_.]*" | sort | uniq -c
+	cuobjdump -sass torchacc_b200/_C.so | grep -oE "[HQ]GMMA[A-Z0-9.]*|UTMA[A-Z0-9.]*|UBLKCP[A-Z0-9.]*|USETMAXREG[A-Z0-9_.]*" | sort | uniq -c
 
 # compute-sanitizer over the hand-written kernels (the reference has no sanitizer hooks at all, SURVEY 5.2):
-# memcheck + synccheck on the stand-alone GEMM harness (every descriptor / TMA / TMEM path, static and dynamic tile
+# memcheck + synccheck on the stand-alone GEMM harness (every descriptor / TMA path, static and dynamic tile
 # scheduling) and memcheck on the op-level numerics tests.
 sanitize: build
 	compute-sanitizer --tool memcheck --error-exitcode 1 build/gemm_test 3 0 1
 	compute-sanitizer --tool synccheck --error-exitcode 1 build/gemm_test 2 0 1
 	compute-sanitizer --tool memcheck --error-exitcode 1 $(PY) -m pytest tests/test_ops_gpu.py -q -m gpu -k "rmsnorm or swiglu or rope or cross_entropy or adamw"
-	compute-sanitizer --tool synccheck $(PY) tools/ncu_targets.py      # MX-FP8 GEMM, SwiGLU epilogue, blockwise / dropout attention
 
 # peer-memory collectives under the sanitizer on 2 GPUs: NCCL-free self check (NCCL's own kernels abort a synccheck run)
 sanitize-multigpu: build

@@ -1,12 +1,16 @@
 #!/usr/bin/env python
-"""Flagship benchmark: Llama-3-8B, FSDP (ZeRO-3) + gradient checkpointing, bf16, seq 4096, synthetic tokens.
+"""Flagship benchmark: Llama-3 family, FSDP (ZeRO-3) + gradient checkpointing, bf16, seq 4096, synthetic tokens.
+
+The default model is Llama-3.2-1B: parameters, fp32 master copy and AdamW state (16 bytes per parameter) plus the
+activations of 2 x 4096 tokens fit the 80 GB of one H100.  ``--model llama3-8b`` needs 8 GPUs' worth of sharding.
 
     python bench.py --gpus N --steps K --warmup W            # ours (torchrun launches N ranks for N > 1)
     python bench.py --impl reference --gpus N ...            # unmodified reference from baseline/_ref
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as DIR/*.npy
 
 Metric (BASELINE.json): training tokens/s for the WHOLE job, device-timed with CUDA events, max over ranks.
 Weak scaling: the per-GPU batch is fixed (``--mbs``, default 2 sequences of 4096 tokens).
-Each timed step = forward + backward + global grad-norm clip + AdamW update (nothing skipped, full 32 layers).
+Each timed step = forward + backward + global grad-norm clip + AdamW update (nothing skipped, every layer).
 One JSON line is printed by rank 0.
 """
 from __future__ import annotations
@@ -16,6 +20,7 @@ import json
 import os
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
@@ -40,7 +45,7 @@ def parse():
     p.add_argument("--hf", action="store_true",
                    help="ours: run the SAME HuggingFace LlamaForCausalLM object as the reference arm through "
                         "ta.accelerate (kernel patches + FSDP engine) instead of the native model definition")
-    p.add_argument("--model", default="llama3-8b")
+    p.add_argument("--model", default="llama3.2-1b")
     p.add_argument("--seq-len", type=int, default=4096)
     p.add_argument("--mbs", type=int, default=2, help="sequences per GPU per step")
     p.add_argument("--layers", type=int, default=None, help="debug only: override the layer count (invalidates the number)")
@@ -48,9 +53,16 @@ def parse():
     p.add_argument("--attn", default=None, help="attention backend override (native|sdpa)")
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--trace", default=None, help="write a kernel timeline (chrome trace) of one extra, untimed step")
+    p.add_argument("--dump-outputs", default=None, metavar="DIR",
+                   help="after the timed steps write what the last timed step returned to its caller as "
+                        "DIR/<name>.npy (float32): loss, grad_norm and a fixed seeded sample of the updated parameters "
+                        "(rank 0's values and, for N > 1, rank 0's parameter shards).  Only with --impl ours")
     p.add_argument("--no-comm-trace", action="store_true",
                    help="skip the extra profiled step that measures exposed communication when N > 1")
-    return p.parse_args()
+    a = p.parse_args()
+    if a.dump_outputs and a.impl != "ours":
+        p.error("--dump-outputs is implemented for --impl ours only")
+    return a
 
 
 class ClockSampler:
@@ -89,23 +101,52 @@ class ClockSampler:
 
 
 def bench_config(a, world, layers):
-    """The ``config`` object of the JSON line: identical in every arm (the driver compares them)."""
+    """The ``config`` object of the JSON line: identical in every arm (so that they can be compared)."""
     return {"model": a.model, "global_batch": a.mbs * world, "seq_len": a.seq_len,
             "parallelism": f"fsdp{world}" + ("" if a.no_gc else "+gc"), "layers": layers,
-            "l2": "no explicit flush: each step streams >16 GB of weights/activations (>> 126 MB L2)"}
+            "l2": "no explicit flush: each step streams several GB of weights/activations (>> 50 MB L2)"}
 
 
-METRIC = "Llama-3-8B FSDP bf16 training throughput (whole job, device-timed, max over ranks)"
+def metric(a):
+    return f"{a.model} FSDP bf16 training throughput (whole job, device-timed, max over ranks)"
+
+
+def vs_a100(a, value, world):
+    """Ratio to the published A100 figure, which exists for Llama-3-8B only."""
+    return value / (A100_TOKENS_PER_S_PER_GPU * world) if a.model == "llama3-8b" else None
+
+
+def dump_outputs(path, last, model):
+    """What the caller of the last timed step received: the loss, the global gradient norm returned by the clip, and the
+    parameters the optimizer left behind (4096 entries per tensor at fixed, seeded positions)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    g = torch.Generator().manual_seed(4321)
+    parts = []
+    for prm in model.parameters():
+        flat = prm.detach().reshape(-1)
+        if flat.numel() == 0:
+            continue
+        idx = torch.randint(0, flat.numel(), (min(flat.numel(), 4096),), generator=g)
+        parts.append(flat[idx.to(flat.device)].float().cpu())
+    for name, t in (("loss", last["loss"]), ("grad_norm", torch.as_tensor(last["grad_norm"]))):
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().reshape(1).cpu().numpy())
+    np.save(os.path.join(path, "params_sample.npy"), torch.cat(parts).numpy())
 
 
 def hf_llama(a, torch, device, world):
-    """HuggingFace Llama-3-8B (random init, same distributions as the native arm) -- the model object the reference
-    arm, the torch_fsdp arm and ``--hf`` all run."""
+    """HuggingFace Llama of the ``--model`` geometry (random init, same distributions as the native arm) -- the model
+    object the reference arm, the torch_fsdp arm and ``--hf`` all run."""
     from transformers import LlamaConfig, LlamaForCausalLM
-    hf = LlamaConfig(vocab_size=128256, hidden_size=4096, intermediate_size=14336,
-                     num_hidden_layers=a.layers or 32, num_attention_heads=32, num_key_value_heads=8,
-                     max_position_embeddings=max(a.seq_len, 8192), rope_theta=500000.0, rms_norm_eps=1e-5,
-                     tie_word_embeddings=False, attn_implementation="flash_attention_2", use_cache=False)
+    from torchacc_b200.models import llama_config
+    m = llama_config(a.model)
+    hf = LlamaConfig(vocab_size=m.vocab_size, hidden_size=m.hidden_size, intermediate_size=m.intermediate_size,
+                     num_hidden_layers=a.layers or m.num_hidden_layers, num_attention_heads=m.num_attention_heads,
+                     num_key_value_heads=m.num_key_value_heads, head_dim=m.head_dim,
+                     max_position_embeddings=max(a.seq_len, 8192), rope_theta=m.rope_theta, rms_norm_eps=m.rms_norm_eps,
+                     tie_word_embeddings=m.tie_word_embeddings, attn_implementation="flash_attention_2",
+                     use_cache=False)
     torch.manual_seed(1234)
     with torch.device("meta"):
         model = LlamaForCausalLM(hf)
@@ -172,7 +213,7 @@ def run_ours(a):
     if a.hf:
         if world > 1:
             ta.dist.init_process_group()
-        model, _ = hf_llama(a, torch, device, 1)        # built on the device: 16 GB of bf16 per rank
+        model, _ = hf_llama(a, torch, device, 1)        # built on the device
         model = model.to(torch.bfloat16)
     else:
         with torch.device(device):
@@ -212,7 +253,7 @@ def run_ours(a):
         out = model(**batch)
         loss = out["loss"]
         loss.backward()
-        model.clip_grad_norm_(1.0)
+        last["grad_norm"] = model.clip_grad_norm_(1.0)
         opt.step()
         model.zero_grad()
         last["loss"] = loss
@@ -231,6 +272,8 @@ def run_ours(a):
     clocks = sampler.stop() if sampler else None
     tokens = a.mbs * a.seq_len * world * a.steps
     value = tokens / (ms / 1e3)
+    if a.dump_outputs and rank == 0:
+        dump_outputs(a.dump_outputs, last, model)     # before the untimed steps below move the state on
 
     # ---- end-to-end through the public API: AsyncLoader H2D every step + loss D2H every step ---------------------
     e2e = None
@@ -260,7 +303,7 @@ def run_ours(a):
     if a.trace or (world > 1 and not a.no_comm_trace):
         # one extra step under the CUPTI-based torch profiler, AFTER every timed region (never part of a number):
         # gives the exposed-communication figure of BASELINE.json's metric (communication-kernel time not hidden
-        # behind compute kernels, rank 0's timeline).  tools/trace_summary.py prints the full tables for profiles/.
+        # behind compute kernels, rank 0's timeline).  tools/trace_summary.py prints the full tables.
         # every rank runs exactly one more step whatever happens to the profiler (a rank that skipped it would
         # leave its peers waiting inside the collectives)
         prof = None
@@ -279,7 +322,7 @@ def run_ours(a):
                 if rank != 0 and a.trace and os.environ.get("TORCHACC_B200_TRACE_ALL", "0") == "1":
                     prof.export_chrome_trace(a.trace.replace(".json", f".rank{rank}.json"))   # skew diagnostics
                 if rank == 0:
-                    path = a.trace or os.path.join("/tmp", f"tb_bench_trace_{os.getpid()}.json")
+                    path = a.trace or os.path.join(tempfile.gettempdir(), f"tb_bench_trace_{os.getpid()}.json")
                     os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
                     prof.export_chrome_trace(path)
                     sys.path.insert(0, os.path.join(ROOT, "tools"))
@@ -313,16 +356,16 @@ def run_ours(a):
         pass
     if rank == 0:
         res = {
-            "metric": METRIC,
+            "metric": metric(a),
             "value": value, "unit": "tokens/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
             "ms_per_step": ms / a.steps, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": value / (A100_TOKENS_PER_S_PER_GPU * world),
+            "vs_baseline": vs_a100(a, value, world),
             "dtype": "mxfp8 linears (e4m3 + ue8m0/32), bf16 elsewhere" if a.fp8 else "bf16", "data": "synthetic",
             "impl": "ours",
             "config": dict(bench_config(a, world, mcfg.num_hidden_layers), **({"fp8": True} if a.fp8 else {})),
             "detail": {"model_code": "HF LlamaForCausalLM through ta.accelerate" if a.hf else "native build_llama",
                        "optimizer": "FusedAdamW + clip_grad_norm(1.0)", "attention": ta.ops.get_attention_backend(),
-                       "stack": "torchacc_b200: own FSDP engine + tcgen05 GEMM/attention + symmetric-memory collectives",
+                       "stack": "torchacc_b200: own FSDP engine + wgmma GEMM/attention + symmetric-memory collectives",
                        "engine_stats": dict(getattr(getattr(model, "engine", None), "stats", {}) or {}),
                        "carried_collectives": carry_counters},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches, "comm": comm,
@@ -415,7 +458,7 @@ def run_reference(a):
         unavailable(msg[:400])
 
     g = torch.Generator().manual_seed(rank)
-    host = torch.randint(0, 128256, (a.mbs, a.seq_len), generator=g).pin_memory()
+    host = torch.randint(0, hf.vocab_size, (a.mbs, a.seq_len), generator=g).pin_memory()
     ids = host.to(device)
     last = {}
 
@@ -455,10 +498,10 @@ def run_reference(a):
                "h2d_bytes_per_step": int(a.mbs * a.seq_len * 8), "d2h_bytes_per_step": 4, "last_loss": loss_val}
     if rank == 0:
         print(json.dumps({
-            "metric": METRIC,
+            "metric": metric(a),
             "value": value, "unit": "tokens/s", "n_gpus": world, "steps": a.steps, "warmup": a.warmup,
             "ms_per_step": ms / a.steps, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": value / (A100_TOKENS_PER_S_PER_GPU * world), "dtype": "bf16", "data": "synthetic",
+            "vs_baseline": vs_a100(a, value, world), "dtype": "bf16", "data": "synthetic",
             "impl": "reference",
             "config": bench_config(a, world, hf.num_hidden_layers),
             "detail": {"model_code": "HF LlamaForCausalLM", "gc": "HF gradient_checkpointing_enable()",
@@ -501,7 +544,7 @@ def run_torch_fsdp(a):
     os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
     os.environ.setdefault("MASTER_PORT", "29533")
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=device)
-    model, hf = hf_llama(a, torch, device, 1)          # built on the GPU (32 GB fp32), FSDP shards it from there
+    model, hf = hf_llama(a, torch, device, 1)          # built on the GPU in fp32, FSDP shards it from there
     for m in model.modules():
         if type(getattr(m, "act_fn", None)).__name__ == "SiLUActivation":
             m.act_fn = torch.nn.SiLU()
@@ -522,7 +565,7 @@ def run_torch_fsdp(a):
                  device_id=torch.cuda.current_device(), sync_module_states=False)
     opt = torch.optim.AdamW(model.parameters(), lr=1e-5, betas=(0.9, 0.95), weight_decay=0.1, fused=True)
     g = torch.Generator().manual_seed(rank)
-    host = torch.randint(0, 128256, (a.mbs, a.seq_len), generator=g).pin_memory()
+    host = torch.randint(0, hf.vocab_size, (a.mbs, a.seq_len), generator=g).pin_memory()
     ids = host.to(device)
     last = {}
 
@@ -559,9 +602,9 @@ def run_torch_fsdp(a):
                "h2d_bytes_per_step": int(a.mbs * a.seq_len * 8), "d2h_bytes_per_step": 4, "last_loss": loss_val}
     if rank == 0:
         print(json.dumps({
-            "metric": METRIC, "value": value, "unit": "tokens/s", "n_gpus": world, "steps": a.steps,
+            "metric": metric(a), "value": value, "unit": "tokens/s", "n_gpus": world, "steps": a.steps,
             "warmup": a.warmup, "ms_per_step": ms / a.steps, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": value / (A100_TOKENS_PER_S_PER_GPU * world), "dtype": "bf16", "data": "synthetic",
+            "vs_baseline": vs_a100(a, value, world), "dtype": "bf16", "data": "synthetic",
             "impl": "torch_fsdp", "config": bench_config(a, world, hf.num_hidden_layers),
             "detail": {"note": "NOT the reference arm: hand-assembled torch FSDP1 stack mirroring reference "
                                "dist/fsdp.py:196-216 so that N > 1 has a same-box competitor",

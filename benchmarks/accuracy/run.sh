@@ -1,5 +1,5 @@
 #!/usr/bin/env bash
-# Accuracy benchmark (counterpart of reference benchmarks/accuracy/run.sh): train the same model with the sm_100a
+# Accuracy benchmark (counterpart of reference benchmarks/accuracy/run.sh): train the same model with the sm_90a
 # kernels and with the plain-PyTorch reference ops, then assert |delta train_loss| <= 1e-2.
 #   NPROC=1 MODEL=llama3.2-1b STEPS=200 bash benchmarks/accuracy/run.sh
 #   HF=1 ...      the HuggingFace LlamaForCausalLM of the same geometry through ta.accelerate (the object the reference's

@@ -3,7 +3,7 @@
 benchmarks/accuracy/run_clm.py + llama.sh: HF run_clm on Llama-3.2-1B / wikitext, torch-native vs torchacc).
 
 Two arms, selected with ``--impl``:
-  native   : torchacc_b200 on its sm_100a kernels (tcgen05 GEMM, flash attention, fused norm/rope/swiglu/CE/AdamW)
+  native   : torchacc_b200 on its sm_90a kernels (wgmma GEMM, flash attention, fused norm/rope/swiglu/CE/AdamW)
   torch    : the SAME framework code with ``TORCHACC_B200_DISABLE_NATIVE=1`` -> every op runs its plain PyTorch
              reference on the GPU (or CPU)
 Both arms share model init, data order and hyper-parameters; the final ``train_loss`` (mean over the last

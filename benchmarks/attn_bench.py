@@ -1,4 +1,4 @@
-"""Attention micro-benchmark: our tcgen05 kernels vs the library paths (torch SDPA / flash-attn 2) on the Llama-3-8B
+"""Attention micro-benchmark: our wgmma kernels vs the library paths (torch SDPA / flash-attn 2) on the Llama-3-8B
 attention shape.  CUDA-event timing, L2 flushed between iterations."""
 import argparse
 import json

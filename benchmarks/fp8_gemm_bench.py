@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""MX-FP8 vs bf16 tcgen05 GEMM on the four Llama-3-8B linear shapes (T = 8192 tokens), plus the quantiser cost.
-CUDA-event timing, 20 iterations after 5 warm-up runs, operands rotated over > 126 MB so L2 does not hold them."""
+"""MX-FP8 vs bf16 wgmma GEMM on the four Llama-3-8B linear shapes (T = 8192 tokens), plus the quantiser cost.
+CUDA-event timing, 20 iterations after 5 warm-up runs, operands rotated over > 50 MB so L2 does not hold them."""
 import json
 import os
 import sys
@@ -31,7 +31,7 @@ def main():
     shapes = [("qkv", T, 6144, 4096), ("o", T, 4096, 4096), ("gate_up", T, 28672, 4096), ("down", T, 4096, 14336)]
     rows = []
     for name, M, N, K in shapes:
-        reps = max(2, int(300e6 // ((M + N) * K * 2)) + 1)          # rotate operand sets: > 126 MB touched
+        reps = max(2, int(300e6 // ((M + N) * K * 2)) + 1)          # rotate operand sets: > 50 MB (the L2 size) touched
         A = [(torch.randn(M, K, device=dev) * 0.5).bfloat16() for _ in range(reps)]
         B = [(torch.randn(N, K, device=dev) * 0.05).bfloat16() for _ in range(reps)]
         out = torch.empty(M, N, dtype=torch.bfloat16, device=dev)

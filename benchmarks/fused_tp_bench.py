@@ -4,7 +4,7 @@
 
 Per op: device time (CUDA events, L2 flushed between iterations, max over ranks) of
   fused   : one kernel (all-gather->GEMM) / GEMM with peer-store epilogue + reduce kernel (GEMM->reduce-scatter)
-  unfused : NCCL all_gather_into_tensor / reduce_scatter_tensor + the same tcgen05 GEMM
+  unfused : NCCL all_gather_into_tensor / reduce_scatter_tensor + the same wgmma GEMM
   gemm    : the GEMM alone (lower bound: perfect overlap)
 """
 import argparse
@@ -90,9 +90,10 @@ def main():
         err = float((of.float() - out.float()).abs().max())
         res.append(dict(op="gemm_rs", layer=name, M=T, N=H, K=K, fused_ms=t_f, unfused_ms=t_u, gemm_only_ms=t_g,
                         speedup=t_u / t_f, tflops_fused=2.0 * T * H * K / t_f / 1e9, max_abs_err=err))
-    # roofline per the profiling recipe: target time = the slower of FLOPs / measured GEMM peak and the bytes that must
-    # cross NVLink / measured link bandwidth (770 GB/s per direction per GPU)
-    peak_tf, link_gbs = 1689.8, 770.0
+    # roofline per the profiling recipe: target time = the slower of FLOPs / GEMM peak and the bytes that must
+    # cross NVLink / link bandwidth (H100 SXM data sheet: 989 TFLOP/s dense bf16, 450 GB/s per direction per GPU;
+    # MEASURED_PEAKS.json, when present, replaces the compute figure with a measured one)
+    peak_tf, link_gbs = 989.0, 450.0
     try:
         mp = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))
         peak_tf = float(mp.get("bf16_tflops", peak_tf))

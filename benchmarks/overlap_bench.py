@@ -1,4 +1,4 @@
-"""How much does a collective running on a side stream slow down the tcgen05 GEMM?  (2+ GPUs)
+"""How much does a collective running on a side stream slow down the wgmma GEMM?  (2+ GPUs)
 
     torchrun --nproc-per-node 2 benchmarks/overlap_bench.py
 

@@ -1,24 +1,21 @@
-// FlashAttention backward on tcgen05 / TMEM / TMA for sm_100a.
+// FlashAttention backward on wgmma / TMA for sm_90a.
 //
-// One CTA per (128-key tile, kv head, batch); it loops over the q heads of the GQA group and over the query tiles
-// that can see this key tile, so dK/dV are accumulated in TMEM with no atomics.  The score tile is computed
-// TRANSPOSED (S^T = K Q^T: TMEM lanes = keys, columns = queries), which lets every later GEMM read its operands in
-// place:
-//   (a) S^T  = K  Q^T    A = K  (smem, K-major)          B = Q  (smem, K-major)      -> TMEM R0
-//   (b) dP^T = V  dO^T   A = V  (smem, K-major)          B = dO (smem, K-major)      -> TMEM R1
-//   softmax warps (thread = key row):  P^T = exp2(S^T*scale - LSE), dS^T = P^T o (dP^T - delta) * scale
-//        P^T  -> TMEM R0 (bf16, aliases S^T)      dS^T -> smem (bf16, 128B-swizzled rows)
-//   (e) dQ   = dS K      A = dS^T smem read MN-major     B = K  (smem, MN-major)     -> TMEM R1 (aliases dP^T)
-//   (c) dV  += P^T dO    A = P^T (TMEM)                  B = dO (smem, MN-major)     -> TMEM R2
-//   (d) dK  += dS^T Q    A = dS^T (smem, K-major)        B = Q  (smem, MN-major)     -> TMEM R3
-// dQ is reduced across key tiles with TMA bulk reduce-add (cp.reduce.async.bulk.tensor .add.f32) from a swizzled smem
-// staging tile that reuses the dS^T buffer -- per-lane red.global atomics cap at ~1 lane/clk/SM and were 80% of the
-// first version's run time.
-// Q/dO tiles stream through a 2-stage TMA ring; K/V stay resident.  The tensor pipe executes MMAs in issue order,
-// so the TMEM/smem aliases above need no extra barriers beyond "softmax done" / "dQ read out".
+// One CTA per (128-key tile, kv head, batch); it loops over the q heads of the GQA group and over the 64-row query
+// tiles that can see this key tile, so dK/dV are accumulated in registers with no atomics.  Two MMA warpgroups own 64
+// keys each and never wait for one another.  The score tile is computed TRANSPOSED (S^T = K Q^T: accumulator rows =
+// keys, columns = queries), which lets every later GEMM take its operands in place:
+//   (a) S^T  = K  Q^T    A = K  (smem, K-major)          B = Q  (smem, K-major)
+//   (b) dP^T = V  dO^T   A = V  (smem, K-major)          B = dO (smem, K-major)
+//   in registers:  P^T = exp2(S^T*scale - LSE), dS^T = P^T o (dP^T - delta) * scale
+//   (c) dV  += P^T dO    A = P^T  (registers)            B = dO (smem, MN-major)
+//   (d) dK  += dS^T Q    A = dS^T (registers)            B = Q  (smem, MN-major)
+//   (e) dQ   = dS K      A = dS^T (smem, read MN-major)  B = K  (smem, MN-major), over the warpgroup's 64 keys
+// dQ partial tiles are reduced into the fp32 accumulator with vector red.global.add.
+// Q/dO tiles stream through a 2-stage TMA ring; K/V stay resident.
 //
 // Reference parity: FA2 backward reached by reference torchacc/ops/flash_attn.py:56,152,206,252,301.
 #include <math.h>
+#include <stdio.h>
 
 #include "../common/ptx.cuh"
 #include "../common/tensormap.h"
@@ -27,8 +24,9 @@
 
 namespace tb {
 
-constexpr int kTile = 128;
-constexpr int kBwdThreads = 384;  // 4 control warps + 2 softmax warpgroups (each owns 64 of the 128 query columns)
+constexpr int kTile = 128;        // keys per CTA
+constexpr int kQTile = 64;        // query rows per iteration
+constexpr int kBwdThreads = 384;  // producer warpgroup + 2 MMA warpgroups (64 keys each)
 constexpr int kQStages = 2;
 
 struct BwdArgs {
@@ -51,41 +49,33 @@ struct BwdArgs {
   long long* trace;   // optional [64 iterations][16 slots] clock64 stamps of CTA (0,0,0) (debug / profiling)
 };
 
-#define TB_TRACE(slot)                                                                             \
-  do {                                                                                             \
-    if (args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && it < 64) \
-      args.trace[it * 16 + (slot)] = clock64();                                                    \
-  } while (0)
-
 template <int D>
 struct BwdSmem {
   static constexpr int kChunks = D / 64;
-  static constexpr int kTileBytes = kTile * D * 2;
+  static constexpr int kKVBytes = kTile * D * 2;
+  static constexpr int kQBytes = kQTile * D * 2;
   static constexpr int kK = 0;
-  static constexpr int kV = kK + kTileBytes;
-  static constexpr int kQ = kV + kTileBytes;
-  static constexpr int kDO = kQ + kQStages * kTileBytes;
-  static constexpr int kDS = kDO + kQStages * kTileBytes;
-  static constexpr int kStat = kDS + kTile * kTile * 2;  // lse2[128], delta[128]
-  static constexpr int kBar = kStat + 2 * kTile * 4;
+  static constexpr int kV = kK + kKVBytes;
+  static constexpr int kQ = kV + kKVBytes;
+  static constexpr int kDO = kQ + kQStages * kQBytes;
+  static constexpr int kDS = kDO + kQStages * kQBytes;      // dS^T [128 keys][64 queries], one 128-byte row per key
+  static constexpr int kStat = kDS + kTile * kQTile * 2;    // per warpgroup: lse2[64], delta[64]
+  static constexpr int kBar = kStat + 2 * 2 * kQTile * 4;
   static constexpr int kTotal = kBar + 128 + 1024;
 };
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
 template <int D, bool kBf16, bool kDrop>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
-                 const __grid_constant__ CUtensorMap tmap_dq, const BwdArgs args) {
+                 const BwdArgs args) {
   using S = BwdSmem<D>;
   constexpr int kChunks = S::kChunks;
-  constexpr uint32_t kIdescST = make_idesc_f16(kTile, kTile, Major::K, Major::K, kBf16);   // (a), (b)
-  constexpr uint32_t kIdescDQ = make_idesc_f16(kTile, D, Major::MN, Major::MN, kBf16);     // (e)
-  constexpr uint32_t kIdescDKV = make_idesc_f16(kTile, D, Major::K, Major::MN, kBf16);     // (c), (d)
-  constexpr uint32_t R0 = 0, R1 = 128, R2 = 256, R3 = 384;
+  constexpr int kQChunk = kQTile * 128;   // bytes of one 64-column chunk of a Q / dO stage
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const uint32_t lane = lane_id();
@@ -105,11 +95,9 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int n_last = min(n0 + kTile, k_len) - 1;
   const int i_lo = (wr_eff < 0) ? 0 : max(0, n0 - shift - wr_eff);
   const int i_hi = (args.wl < 0) ? (q_len - 1) : min(q_len - 1, n_last - shift + args.wl);
-  const int it_lo = i_lo / kTile;
-  const int n_qt = (i_hi < i_lo) ? 0 : (i_hi / kTile - it_lo + 1);
+  const int it_lo = i_lo / kQTile;
+  const int n_qt = (i_hi < i_lo) ? 0 : (i_hi / kQTile - it_lo + 1);
   const int n_iter = n_qt * group;
-
-  const int key = n0 + (int)(((warp_idx & 3) * 32) + lane);  // key index owned by a softmax thread
 
   if (n_iter == 0) {  // no query sees these keys: dK = dV = 0
     for (int r = threadIdx.x; r < min(kTile, k_len - n0); r += blockDim.x) {
@@ -123,47 +111,31 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sK = base + S::kK, sV = base + S::kV, sQ = base + S::kQ, sDO = base + S::kDO, sDS = base + S::kDS;
-  float* stat = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + S::kStat);
+  float* stat_all = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + S::kStat);
   const uint32_t bar = base + S::kBar;
   const uint32_t kv_full = bar;
   auto qdo_full = [&](int s) { return bar + 8u * (1 + s); };
-  auto qdo_empty = [&](int s) { return bar + 8u * (3 + s); };
-  const uint32_t s_full = bar + 8u * 5, pds_ready = bar + 8u * 6, dq_full = bar + 8u * 7, r1_free = bar + 8u * 8;
-  const uint32_t dkv_full = bar + 8u * 9, dp_full = bar + 8u * 10;
-  auto qs_free = [&](int s) { return bar + 8u * (11 + s); };   // Q stage no longer read by the dQ bulk reduce
-  const uint32_t tmem_slot = bar + 8u * 13;
+  auto qdo_empty = [&](int s) { return bar + 8u * (1 + kQStages + s); };
 
   if (warp_idx == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v); tma_prefetch_desc(&tmap_do);
-    tma_prefetch_desc(&tmap_dq);
   }
   if (warp_idx == 1 && lane == 0) {
     mbar_init(kv_full, 1);
-    for (int s = 0; s < kQStages; ++s) { mbar_init(qdo_full(s), 1); mbar_init(qdo_empty(s), 1); }
-    mbar_init(s_full, 1);
-    mbar_init(dp_full, 1);
-    for (int s = 0; s < kQStages; ++s) mbar_init(qs_free(s), 2);
-    mbar_init(pds_ready, 8);
-    mbar_init(dq_full, 1);
-    mbar_init(r1_free, 8);
-    mbar_init(dkv_full, 1);
+    for (int s = 0; s < kQStages; ++s) { mbar_init(qdo_full(s), 1); mbar_init(qdo_empty(s), 2); }
     fence_mbar_init();
   }
-  if (warp_idx == 2) tmem_alloc<1>(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
   // iteration -> (q head, q tile): heads outer, tiles inner
   auto iter_head = [&](int it) { return hk * group + it / n_qt; };
-  auto iter_m0 = [&](int it) { return (it_lo + it % n_qt) * kTile; };
+  auto iter_m0 = [&](int it) { return (it_lo + it % n_qt) * kQTile; };
 
-  if (warp_idx == 0) {
+  if (warp_idx < 4) {
+    setmaxnreg_dec<24>();
     // ================================ TMA producer ================================
-    if (lane == 0) {
-      mbar_arrive_expect_tx(kv_full, 2 * S::kTileBytes);
+    if (warp_idx == 0 && lane == 0) {
+      mbar_arrive_expect_tx(kv_full, 2 * S::kKVBytes);
 #pragma unroll
       for (int c = 0; c < kChunks; ++c) {
         tma_load_3d(sK + c * 16384, &tmap_k, kv_full, c * 64, hk, k_start + n0);
@@ -172,306 +144,192 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       for (int it = 0; it < n_iter; ++it) {
         const int s = it % kQStages;
         mbar_wait(qdo_empty(s), ((it / kQStages) & 1) ^ 1);
-        mbar_wait(qs_free(s), ((it / kQStages) & 1) ^ 1);   // Q stage doubles as dQ staging for the bulk reduce
-        mbar_arrive_expect_tx(qdo_full(s), 2 * S::kTileBytes);
+        mbar_arrive_expect_tx(qdo_full(s), 2 * S::kQBytes);
         const int h = iter_head(it), row0 = q_start + iter_m0(it);
 #pragma unroll
         for (int c = 0; c < kChunks; ++c) {
-          tma_load_3d(sQ + s * S::kTileBytes + c * 16384, &tmap_q, qdo_full(s), c * 64, h, row0);
-          tma_load_3d(sDO + s * S::kTileBytes + c * 16384, &tmap_do, qdo_full(s), c * 64, h, row0);
+          tma_load_3d(sQ + s * S::kQBytes + c * kQChunk, &tmap_q, qdo_full(s), c * 64, h, row0);
+          tma_load_3d(sDO + s * S::kQBytes + c * kQChunk, &tmap_do, qdo_full(s), c * 64, h, row0);
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ================================ MMA issuer ================================
-    if (lane == 0) {
-      mbar_wait(kv_full, 0);
-      for (int it = 0; it < n_iter; ++it) {
-        const int s = it % kQStages;
-        const uint32_t q_s = sQ + s * S::kTileBytes, do_s = sDO + s * S::kTileBytes;
-        mbar_wait(qdo_full(s), (it / kQStages) & 1);
-        tc_fence_after();
-        TB_TRACE(0);
-        // (a) S^T = K Q^T -> R0   (in-order pipe: runs after (c) of the previous iteration consumed P^T in R0)
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_ss_f16<1>(tmem_base + R0, desc_kmajor_sw128(sK + (kk / 4) * 16384, kk % 4),
-                         desc_kmajor_sw128(q_s + (kk / 4) * 16384, kk % 4), kIdescST, kk != 0);
-        umma_commit(s_full);    // the softmax warps start exponentiating while dP^T is still being produced
-        // (b) dP^T = V dO^T -> R1 (needs dQ of the previous iteration read out of R1)
-        mbar_wait(r1_free, (it & 1) ^ 1);
-        tc_fence_after();
-        TB_TRACE(1);
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk)
-          umma_ss_f16<1>(tmem_base + R1, desc_kmajor_sw128(sV + (kk / 4) * 16384, kk % 4),
-                         desc_kmajor_sw128(do_s + (kk / 4) * 16384, kk % 4), kIdescST, kk != 0);
-        umma_commit(dp_full);
-        TB_TRACE(2);
-        // softmax warps: P^T -> R0 (TMEM), dS^T -> smem
-        mbar_wait(pds_ready, it & 1);
-        tc_fence_after();
-        TB_TRACE(3);
-        // (e) dQ = dS K -> R1
-#pragma unroll
-        for (int kk = 0; kk < kTile / 16; ++kk)
-          umma_ss_f16<1>(tmem_base + R1, desc_mnmajor_sw128(sDS, kk, 16384), desc_mnmajor_sw128(sK, kk, 16384),
-                         kIdescDQ, kk != 0);
-        // (d) dK += dS^T Q
-#pragma unroll
-        for (int kk = 0; kk < kTile / 16; ++kk)
-          umma_ss_f16<1>(tmem_base + R3, desc_kmajor_sw128(sDS + (kk / 4) * 16384, kk % 4),
-                         desc_mnmajor_sw128(q_s, kk, 16384), kIdescDKV, (it | kk) != 0);
-        umma_commit(dq_full);   // dQ complete AND dS^T smem no longer read: it becomes the dQ staging tile
-        // (c) dV += P^T dO   (A from TMEM: 16 bf16 of K = 8 columns per step)
-#pragma unroll
-        for (int kk = 0; kk < kTile / 16; ++kk)
-          umma_ts_f16(tmem_base + R2, tmem_base + R0 + kk * 8, desc_mnmajor_sw128(do_s, kk, 16384), kIdescDKV,
-                      (it | kk) != 0);
-        umma_commit(qdo_empty(s));
-        TB_TRACE(4);
-      }
-      umma_commit(dkv_full);
-    }
-  } else if (warp_idx >= 4) {
-    // ================================ softmax / dS / dQ read-out / epilogue ================================
-    // two warpgroups: grp 0 = warps 4-7 owns query columns [0,64), grp 1 = warps 8-11 owns [64,128)
-    const uint32_t q4 = warp_idx & 3;
-    const int grp = (warp_idx - 4) >> 2;
-    const int r = q4 * 32 + lane;  // TMEM lane: key row for S^T/dP^T/dV/dK, query row for dQ
-    const uint32_t lane_off = (q4 * 32u) << 16;
-    const float sl2 = args.scale_log2, sc = args.scale;
-    const bool key_ok = key < k_len;
-    const uint32_t drop_key = kDrop ? drop_key_part(args.drop.seed_hi, (uint32_t)key) : 0u;
-    // group 0 prefetches the row statistics of the next query tile
-    float lse_next = 0.f, delta_next = 0.f;
-    auto fetch_stats = [&](int it) {
-      const int h = iter_head(it), row = iter_m0(it) + r;
+    return;
+  }
+
+  // ================================ MMA warpgroups ================================
+  setmaxnreg_inc<240>();
+  const int wg = (warp_idx >> 2) - 1;
+  const int tid = threadIdx.x & 127;
+  const uint32_t quad = lane & 3;
+  const int kr = wg * 64 + (warp_idx & 3) * 16 + (int)(lane >> 2);   // this thread's key rows in the tile: kr, kr + 8
+  const float sl2 = args.scale_log2, sc = args.scale;
+  float* stat = stat_all + wg * 2 * kQTile;                           // this warpgroup's copy of lse2 / delta
+  const uint32_t sK_w = sK + wg * 8192, sV_w = sV + wg * 8192;        // rows [64 wg, 64 wg + 64) of every 64-column chunk
+  const uint32_t sDS_w = sDS + wg * 8192;
+  auto wg_sync = [&]() {   // named barrier of this warpgroup
+    if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
+  };
+  const bool tracing = args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
+  uint32_t drop_key[2] = {0u, 0u};
+  if constexpr (kDrop) {
+    drop_key[0] = drop_key_part(args.drop.seed_hi, (uint32_t)(n0 + kr));
+    drop_key[1] = drop_key_part(args.drop.seed_hi, (uint32_t)(n0 + kr + 8));
+  }
+
+  float dv[D / 2], dk[D / 2];
+  mbar_wait(kv_full, 0);
+  for (int it = 0; it < n_iter; ++it) {
+    const int s = it % kQStages;
+    const int h = iter_head(it), m0 = iter_m0(it);
+    const uint32_t q_s = sQ + s * S::kQBytes, do_s = sDO + s * S::kQBytes;
+    if (tracing && it < 64) args.trace[it * 16 + 0] = clock64();
+    // row statistics of this query tile (the previous tile's readers are past their dS^T barrier)
+    {
+      const int row = m0 + (tid & 63);
       const bool ok = row < q_len;
-      const float l = ok ? args.lse[(long long)h * args.Tq + q_start + row] : INFINITY;
-      lse_next = (l == -INFINITY) ? INFINITY : l * 1.4426950408889634f;
-      delta_next = ok ? args.delta[(long long)h * args.Tq + q_start + row] : 0.f;
-    };
-    if (grp == 0) fetch_stats(0);
-    for (int it = 0; it < n_iter; ++it) {
-      const int h = iter_head(it), m0 = iter_m0(it);
-      // publish this tile's row statistics (all 256 softmax threads finished the previous tile's reads)
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      if (grp == 0) {
-        stat[r] = lse_next;
-        stat[kTile + r] = delta_next;
+      const long long off = (long long)h * args.Tq + q_start + row;
+      if (tid < 64) {
+        const float l = ok ? args.lse[off] : INFINITY;
+        stat[tid] = (l == -INFINITY) ? INFINITY : l * 1.4426950408889634f;
+      } else {
+        stat[tid] = ok ? args.delta[off] : 0.f;
       }
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      mbar_wait(s_full, it & 1);
-      tc_fence_after();
-      if (warp_idx == 4 && lane == 0) TB_TRACE(5);
-      const float slope_l2 = args.alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
-      // interior tile: every query row of the tile sees every key of the tile -> no per-element mask
-      bool interior = (m0 + kTile <= q_len) && (n0 + kTile <= k_len);
-      if (interior) {
-        const int pos_first = m0 + shift, pos_last = m0 + kTile - 1 + shift;
-        const int hi_first = (wr_eff < 0) ? (k_len - 1) : min(k_len - 1, pos_first + wr_eff);
-        const int lo_last = (args.wl < 0) ? 0 : max(0, pos_last - args.wl);
-        interior = (hi_first >= n0 + kTile - 1) && (lo_last <= n0);
-      }
-      // ---- phase 1: P^T = exp2(S^T * scale - LSE) for this group's 64 query columns (needs only S^T) ----
-      uint32_t sv[2][32];
-      uint32_t keep_bits[2] = {0xffffffffu, 0xffffffffu};
-      const uint32_t drop_head = kDrop ? drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)) : 0u;
-      tmem_ld_32x32b_x32(tmem_base + lane_off + R0 + (2 * grp) * 32, sv[0]);
-      tmem_ld_32x32b_x32(tmem_base + lane_off + R0 + (2 * grp + 1) * 32, sv[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      asm volatile("bar.sync 2, 256;" ::: "memory");   // both groups read S^T before P^T overwrites its columns
-      tc_fence_after();
-      if (warp_idx == 4 && lane == 0) TB_TRACE(6);
+    }
+    mbar_wait(qdo_full(s), (it / kQStages) & 1);
+    // ---- (a) S^T = K Q^T, (b) dP^T = V dO^T ----
+    float st[kQTile / 2], dpt[kQTile / 2];
+    wgmma_fence_acc(st);
+    wgmma_fence_acc(dpt);
+    wgmma_fence();
 #pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        const int c = 2 * grp + cc;
-        const float4* lse4 = reinterpret_cast<const float4*>(stat + c * 32);
-        if (args.alibi != nullptr) {   // ALiBi: the forward folded -slope * |query position - key| into the scores
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss<kQTile, kBf16, 0, 0>(st, desc_kmajor_sw128(sK_w + (kk / 4) * 16384, kk % 4),
+                                    desc_kmajor_sw128(q_s + (kk / 4) * kQChunk, kk % 4), kk != 0);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float dist = fabsf((float)(m0 + c * 32 + i + shift - key));
-            sv[cc][i] = __float_as_uint(__uint_as_float(sv[cc][i]) - slope_l2 * dist / sl2);
-          }
-        }
-        // branch-free: exponentiate everything (straight-line FFMA + MUFU so the SFU latency pipelines), then zero
-        // the masked entries of boundary tiles with selects
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss<kQTile, kBf16, 0, 0>(dpt, desc_kmajor_sw128(sV_w + (kk / 4) * 16384, kk % 4),
+                                    desc_kmajor_sw128(do_s + (kk / 4) * kQChunk, kk % 4), kk != 0);
+    wgmma_commit();
+    wg_sync();            // statistics visible; every thread of the group is done with the previous dS^T tile
+    wgmma_wait<0>();
+    wgmma_fence_acc(st);
+    wgmma_fence_acc(dpt);
+    if (tracing && it < 64) args.trace[it * 16 + 1] = clock64();
+
+    // ---- P^T = exp2(S^T * scale - LSE), dS^T = P^T o (dP^T - delta) * scale ----
+    const float slope_l2 = args.alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
+    // interior tile: every query row of the tile sees every key of the tile -> no per-element mask
+    bool interior = (m0 + kQTile <= q_len) && (n0 + kTile <= k_len);
+    if (interior) {
+      const int pos_first = m0 + shift, pos_last = m0 + kQTile - 1 + shift;
+      const int hi_first = (wr_eff < 0) ? (k_len - 1) : min(k_len - 1, pos_first + wr_eff);
+      const int lo_last = (args.wl < 0) ? 0 : max(0, pos_last - args.wl);
+      interior = (hi_first >= n0 + kTile - 1) && (lo_last <= n0);
+    }
+    const uint32_t drop_head = kDrop ? drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)) : 0u;
+    uint32_t pfrag[kQTile / 16][4], dsfrag[kQTile / 16][4];
 #pragma unroll
-        for (int g4 = 0; g4 < 8; ++g4) {
-          const float4 l = lse4[g4];
-          sv[cc][g4 * 4 + 0] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(sv[cc][g4 * 4 + 0]), sl2, -l.x)));
-          sv[cc][g4 * 4 + 1] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(sv[cc][g4 * 4 + 1]), sl2, -l.y)));
-          sv[cc][g4 * 4 + 2] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(sv[cc][g4 * 4 + 2]), sl2, -l.z)));
-          sv[cc][g4 * 4 + 3] = __float_as_uint(fast_exp2(fmaf(__uint_as_float(sv[cc][g4 * 4 + 3]), sl2, -l.w)));
-        }
-        if (!interior) {
+    for (int j = 0; j < kQTile / 8; ++j) {
+      const int c = 8 * j + 2 * (int)quad;                 // query columns c, c + 1 of the tile
+      const float2 l2 = *reinterpret_cast<const float2*>(stat + c);
+      const float2 dl = *reinterpret_cast<const float2*>(stat + kQTile + c);
 #pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int qrow = m0 + c * 32 + i;
+      for (int i = 0; i < 2; ++i) {                        // key rows kr, kr + 8
+        const int key = n0 + kr + 8 * i;
+        float p[2], ds[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int qrow = m0 + c + e;
+          float x = fmaf(st[4 * j + 2 * i + e], sl2, -(e ? l2.y : l2.x));
+          if (args.alibi != nullptr) x -= slope_l2 * fabsf((float)(qrow + shift - key));
+          float pe = fast_exp2(x);
+          if (!interior) {
             const int pos = qrow + shift;
             const int hi = (wr_eff < 0) ? (k_len - 1) : min(k_len - 1, pos + wr_eff);
             const int lo = (args.wl < 0) ? 0 : max(0, pos - args.wl);
-            const bool ok = key_ok && qrow < q_len && key >= lo && key <= hi;
-            sv[cc][i] = ok ? sv[cc][i] : 0u;
+            pe = (key < k_len && qrow < q_len && key >= lo && key <= hi) ? pe : 0.f;
           }
-        }
-        uint32_t pk[16];
-        if constexpr (kDrop) {
-          // dV += (P o mask / (1-p))^T dO: the dropped P^T goes to the tensor core, sv keeps the undropped P^T for dS
-          uint32_t bits = 0;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const uint32_t rowp = drop_row_part(drop_head, (uint32_t)(m0 + c * 32 + i));
-            bits |= (drop_keep(rowp, drop_key, args.drop.thresh24) ? 1u : 0u) << i;
+          float dpe = dpt[4 * j + 2 * i + e];
+          float pv = pe;
+          if constexpr (kDrop) {
+            // dV += (P o mask / (1-p))^T dO; d(dropped P) -> dP: the same mask and 1/(1-p)
+            const bool keep = drop_keep(drop_row_part(drop_head, (uint32_t)qrow), drop_key[i], args.drop.thresh24);
+            pv = keep ? pe * args.drop.rp : 0.f;
+            dpe = keep ? dpe * args.drop.rp : 0.f;
           }
-          keep_bits[cc] = bits;
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float a0 = ((bits >> (2 * i)) & 1u) ? __uint_as_float(sv[cc][2 * i]) * args.drop.rp : 0.f;
-            const float a1 = ((bits >> (2 * i + 1)) & 1u) ? __uint_as_float(sv[cc][2 * i + 1]) * args.drop.rp : 0.f;
-            pk[i] = pack_h2<kBf16>(a0, a1);
-          }
-        } else {
-#pragma unroll
-          for (int i = 0; i < 16; ++i)
-            pk[i] = pack_h2<kBf16>(__uint_as_float(sv[cc][2 * i]), __uint_as_float(sv[cc][2 * i + 1]));
+          p[e] = pv;
+          ds[e] = pe * (dpe - (e ? dl.y : dl.x)) * sc;
         }
-        tmem_st_32x32b_x16(tmem_base + lane_off + R0 + c * 16, pk);   // P^T chunk -> TMEM R0 columns [16c, 16c+16)
+        pfrag[j >> 1][(j & 1) * 2 + i] = pack_h2<kBf16>(p[0], p[1]);
+        const uint32_t dsp = pack_h2<kBf16>(ds[0], ds[1]);
+        dsfrag[j >> 1][(j & 1) * 2 + i] = dsp;
+        // dS^T -> smem row (key), 128B-swizzled: 16-byte unit j of row r lives at unit (j ^ (r & 7))
+        const uint32_t r = (uint32_t)(kr + 8 * i);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sDS + r * 128u + (((uint32_t)j ^ (r & 7u)) << 4) + 4u * quad), "r"(dsp)
+                     : "memory");
       }
-      if (warp_idx == 4 && lane == 0) TB_TRACE(10);   // phase 1 done (P^T stores issued)
-      // ---- the dS^T buffer (and the previous Q stage) were the staging tiles of the previous dQ bulk reduce ----
-      if (it > 0) {
-        if (q4 == 0 && lane == 0) {
-          tma_store_wait_read<0>();
-          mbar_arrive(qs_free((it - 1) % kQStages));
-        }
-        if (grp == 0) asm volatile("bar.sync 3, 128;" ::: "memory"); else asm volatile("bar.sync 4, 128;" ::: "memory");
-      }
-      if (warp_idx == 4 && lane == 0) TB_TRACE(11);   // staging released
-      // ---- phase 2: dS^T = P^T o (dP^T - delta) * scale ----
-      mbar_wait(dp_full, it & 1);
-      tc_fence_after();
-      if (warp_idx == 4 && lane == 0) TB_TRACE(12);
-#pragma unroll
-      for (int cc = 0; cc < 2; ++cc) {
-        const int c = 2 * grp + cc;
-        uint32_t dpv[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + R1 + c * 32, dpv);
-        tmem_ld_wait();
-        const float4* dl4 = reinterpret_cast<const float4*>(stat + kTile + c * 32);
-        if constexpr (kDrop) {   // d(dropped P) -> dP: the same mask and 1/(1-p)
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            dpv[i] = ((keep_bits[cc] >> i) & 1u) ? __float_as_uint(__uint_as_float(dpv[i]) * args.drop.rp) : 0u;
-        }
-        uint32_t dsk[16];
-#pragma unroll
-        for (int g4 = 0; g4 < 8; ++g4) {
-          const float4 dl = dl4[g4];
-          const float d0 = __uint_as_float(sv[cc][g4 * 4 + 0]) * (__uint_as_float(dpv[g4 * 4 + 0]) - dl.x) * sc;
-          const float d1 = __uint_as_float(sv[cc][g4 * 4 + 1]) * (__uint_as_float(dpv[g4 * 4 + 1]) - dl.y) * sc;
-          const float d2 = __uint_as_float(sv[cc][g4 * 4 + 2]) * (__uint_as_float(dpv[g4 * 4 + 2]) - dl.z) * sc;
-          const float d3 = __uint_as_float(sv[cc][g4 * 4 + 3]) * (__uint_as_float(dpv[g4 * 4 + 3]) - dl.w) * sc;
-          dsk[g4 * 2] = pack_h2<kBf16>(d0, d1);
-          dsk[g4 * 2 + 1] = pack_h2<kBf16>(d2, d3);
-        }
-        // dS^T chunk -> smem row r (keys), 64 bytes = 4 x 16B units, 128B-swizzled
-        const uint32_t row_base = sDS + (c >> 1) * 16384 + r * 128;
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const uint32_t unit = (uint32_t)((c & 1) * 4 + u) ^ (uint32_t)(r & 7);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(row_base + unit * 16), "r"(dsk[4 * u]),
-                       "r"(dsk[4 * u + 1]), "r"(dsk[4 * u + 2]), "r"(dsk[4 * u + 3])
-                       : "memory");
-        }
-      }
-      if (warp_idx == 4 && lane == 0) TB_TRACE(13);   // phase 2 compute + smem stores issued
-      tmem_st_wait();
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(pds_ready);
-      if (warp_idx == 4 && lane == 0) TB_TRACE(7);
-      // prefetch the next tile's statistics while the tensor core works
-      if (grp == 0 && it + 1 < n_iter) fetch_stats(it + 1);
-      // ---- dQ tile (lane r = query row m0 + r): TMEM -> swizzled fp32 staging -> ONE round of TMA bulk
-      // reduce-adds per group; nobody waits for them here (the wait sits at the top of the next iteration).
-      // Group g owns D columns [g*D/2, (g+1)*D/2): box 0 is staged in its half of the dS^T buffer, box 1 in its
-      // half of the Q stage (both are dead once (e) and (d) retired).
-      mbar_wait(dq_full, it & 1);
-      tc_fence_after();
-      if (warp_idx == 4 && lane == 0) TB_TRACE(8);
-      constexpr int kBoxes = D / 64;   // 32-column fp32 boxes per group
-      const uint32_t q_stage = sQ + (it % kQStages) * S::kTileBytes;
-#pragma unroll
-      for (int bx = 0; bx < kBoxes; ++bx) {
-        const int col0 = grp * (D / 2) + bx * 32;
-        const uint32_t stage = (bx == 0 ? sDS : q_stage) + grp * 16384;
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + R1 + col0, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-          const uint32_t unit = (uint32_t)u ^ (uint32_t)(r & 7);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(stage + r * 128 + unit * 16), "r"(v[4 * u]),
-                       "r"(v[4 * u + 1]), "r"(v[4 * u + 2]), "r"(v[4 * u + 3])
-                       : "memory");
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(r1_free);        // R1 has been read out: dP^T of the next tile may land
-      if (grp == 0) asm volatile("bar.sync 3, 128;" ::: "memory"); else asm volatile("bar.sync 4, 128;" ::: "memory");
-      if (q4 == 0 && lane == 0) {
-#pragma unroll
-        for (int bx = 0; bx < kBoxes; ++bx)
-          tma_reduce_add_2d(&tmap_dq, (bx == 0 ? sDS : q_stage) + grp * 16384, h * D + grp * (D / 2) + bx * 32,
-                            q_start + m0);
-        tma_store_commit();
-      }
-      if (warp_idx == 4 && lane == 0) TB_TRACE(9);
     }
-    if (q4 == 0 && lane == 0) tma_store_wait<0>();   // all bulk reductions of this thread have landed
-    // ---- epilogue: dV (R2), dK (R3) -> bf16; each group writes half of the D columns ----
-    mbar_wait(dkv_full, 0);
-    tc_fence_after();
-    uint16_t* pdv = args.dv + (long long)(k_start + key) * args.dv_ts + (long long)hk * D;
-    uint16_t* pdk = args.dk + (long long)(k_start + key) * args.dk_ts + (long long)hk * D;
+    fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+    wg_sync();
+    // ---- (c) dV += P^T dO, (d) dK += dS^T Q, (e) dQ = dS K over this warpgroup's keys ----
+    float dq[D / 2];
+    wgmma_fence_acc(dv);
+    wgmma_fence_acc(dk);
+    wgmma_fence_acc(dq);
+    wgmma_fence();
 #pragma unroll
-    for (int which = 0; which < 2; ++which) {
-      uint16_t* dst = which == 0 ? pdv : pdk;
-      const uint32_t reg = which == 0 ? R2 : R3;
+    for (int kk = 0; kk < kQTile / 16; ++kk)
+      wgmma_rs<D, kBf16, 1>(dv, pfrag[kk], desc_mnmajor_sw128(do_s, kk, kQChunk), (it | kk) != 0);
 #pragma unroll
-      for (int cc = 0; cc < D / 64; ++cc) {
-        const int c = grp * (D / 64) + cc;
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + reg + c * 32, v);
-        tmem_ld_wait();
-        if (key_ok) {
+    for (int kk = 0; kk < kQTile / 16; ++kk)
+      wgmma_rs<D, kBf16, 1>(dk, dsfrag[kk], desc_mnmajor_sw128(q_s, kk, kQChunk), (it | kk) != 0);
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            uint4 w;
-            w.x = pack_h2<kBf16>(__uint_as_float(v[8 * u + 0]), __uint_as_float(v[8 * u + 1]));
-            w.y = pack_h2<kBf16>(__uint_as_float(v[8 * u + 2]), __uint_as_float(v[8 * u + 3]));
-            w.z = pack_h2<kBf16>(__uint_as_float(v[8 * u + 4]), __uint_as_float(v[8 * u + 5]));
-            w.w = pack_h2<kBf16>(__uint_as_float(v[8 * u + 6]), __uint_as_float(v[8 * u + 7]));
-            *reinterpret_cast<uint4*>(dst + c * 32 + u * 8) = w;
-          }
-        }
-        __syncwarp();
-      }
+    for (int kk = 0; kk < 64 / 16; ++kk)
+      wgmma_ss<D, kBf16, 1, 1>(dq, desc_mnmajor_sw128(sDS_w, kk, 0), desc_mnmajor_sw128(sK_w, kk, 16384), kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(dv);
+    wgmma_fence_acc(dk);
+    wgmma_fence_acc(dq);
+    if (tid == 0) mbar_arrive(qdo_empty(s));
+    if (tracing && it < 64) args.trace[it * 16 + 2] = clock64();
+    // dQ rows = queries of the tile: reduce this warpgroup's partial sums into the fp32 accumulator
+    const int qr = (warp_idx & 3) * 16 + (int)(lane >> 2);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int row = m0 + qr + 8 * i;
+      if (row >= q_len) continue;
+      float* dst = args.dq_acc + ((long long)(q_start + row) * args.Hq + h) * D + 2 * quad;
+#pragma unroll
+      for (int j = 0; j < D / 8; ++j) red_add_v2(dst + 8 * j, dq[4 * j + 2 * i], dq[4 * j + 2 * i + 1]);
     }
   }
 
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
+  // ---- epilogue: dV, dK -> bf16 / fp16 ----
+  const bool vec_k = (args.dk_ts % 8 == 0) && (reinterpret_cast<uintptr_t>(args.dk) % 16 == 0);
+  const bool vec_v = (args.dv_ts % 8 == 0) && (reinterpret_cast<uintptr_t>(args.dv) % 16 == 0);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int key = n0 + kr + 8 * i;
+    const bool ok = key < k_len;
+    uint16_t* pdv = args.dv + (long long)(k_start + key) * args.dv_ts + (long long)hk * D;
+    uint16_t* pdk = args.dk + (long long)(k_start + key) * args.dk_ts + (long long)hk * D;
+#pragma unroll
+    for (int g = 0; g < D / 32; ++g) {
+      uint32_t xv[4], xk[4];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * g + jj;
+        xv[jj] = pack_h2<kBf16>(dv[4 * j + 2 * i], dv[4 * j + 2 * i + 1]);
+        xk[jj] = pack_h2<kBf16>(dk[4 * j + 2 * i], dk[4 * j + 2 * i + 1]);
+      }
+      quad_transpose(xv, lane);
+      quad_transpose(xk, lane);
+      if (ok) {
+        store_row8(pdv + 32 * g + 8 * quad, xv, 8, vec_v);
+        store_row8(pdk + 32 * g + 8 * quad, xk, 8, vec_k);
+      }
+    }
   }
 }
 
@@ -521,17 +379,18 @@ bwd_convert_dq_kernel(const float* __restrict__ dq_acc, uint16_t* __restrict__ d
 static long long* g_bwd_trace = nullptr;
 void flash_attn_bwd_set_trace(long long* p) { g_bwd_trace = p; }
 
-static CUtensorMap make_map_thd_b(const void* base, long long tokens, int heads, int D, long long ts, bool bf16) {
+static CUtensorMap make_map_thd_b(const void* base, long long tokens, int heads, int D, long long ts, bool bf16,
+                                  int box_rows) {
   uint64_t dims[3] = {(uint64_t)D, (uint64_t)heads, (uint64_t)tokens};
   uint64_t strides[2] = {(uint64_t)D * 2, (uint64_t)ts * 2};
-  uint32_t box[3] = {64, 1, 128};
+  uint32_t box[3] = {64, 1, (uint32_t)box_rows};
   return make_tensor_map(base, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, dims,
                          strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 template <int D, bool kBf16, bool kDrop>
 static cudaError_t launch_bwd(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
-                              const CUtensorMap& mdo, const CUtensorMap& mdq, const BwdArgs& a, int num_k_tiles,
+                              const CUtensorMap& mdo, const BwdArgs& a, int num_k_tiles,
                               cudaStream_t stream) {
   using S = BwdSmem<D>;
   auto kern = flash_bwd_kernel<D, kBf16, kDrop>;
@@ -542,7 +401,7 @@ static cudaError_t launch_bwd(const CUtensorMap& mq, const CUtensorMap& mk, cons
     configured = true;
   }
   dim3 grid(num_k_tiles, a.Hk, a.B);
-  kern<<<grid, kBwdThreads, S::kTotal, stream>>>(mq, mk, mv, mdo, mdq, a);
+  kern<<<grid, kBwdThreads, S::kTotal, stream>>>(mq, mk, mv, mdo, a);
   return cudaGetLastError();
 }
 
@@ -584,18 +443,12 @@ cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const
   // 2) main kernel
   cudaError_t e = cudaSuccess;
   if (phases & 2) {
-  CUtensorMap mq, mk, mv, mdo, mdq;
+  CUtensorMap mq, mk, mv, mdo;
   try {
-    mq = make_map_thd_b(q, Tq, Hq, D, q_ts, is_bf16);
-    mk = make_map_thd_b(k, Tk, Hk, D, k_ts, is_bf16);
-    mv = make_map_thd_b(v, Tk, Hk, D, v_ts, is_bf16);
-    mdo = make_map_thd_b(dout, Tq, Hq, D, do_ts, is_bf16);
-    {  // fp32 dQ accumulator [Tq, Hq*D]: 128 x 32 boxes (128 B rows, SWIZZLE_128B) for the bulk reduce-add
-      uint64_t dims[2] = {(uint64_t)Hq * D, (uint64_t)Tq};
-      uint64_t strides[1] = {(uint64_t)Hq * D * 4};
-      uint32_t box[2] = {32, 128};
-      mdq = make_tensor_map(dq_acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    }
+    mq = make_map_thd_b(q, Tq, Hq, D, q_ts, is_bf16, kQTile);
+    mk = make_map_thd_b(k, Tk, Hk, D, k_ts, is_bf16, kTile);
+    mv = make_map_thd_b(v, Tk, Hk, D, v_ts, is_bf16, kTile);
+    mdo = make_map_thd_b(dout, Tq, Hq, D, do_ts, is_bf16, kQTile);
   } catch (const std::exception& e) {
     fprintf(stderr, "%s\n", e.what());
     return cudaErrorInvalidValue;
@@ -628,8 +481,8 @@ cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const
     a.drop = DropoutParams{0u, 1.f, 0u, 0u};
   }
 #define TB_BWD(DD, BF)                                                                            \
-  (drop ? launch_bwd<DD, BF, true>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream)                  \
-        : launch_bwd<DD, BF, false>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream))
+  (drop ? launch_bwd<DD, BF, true>(mq, mk, mv, mdo, a, num_k_tiles, stream)                  \
+        : launch_bwd<DD, BF, false>(mq, mk, mv, mdo, a, num_k_tiles, stream))
   if (is_bf16) e = (D == 128) ? TB_BWD(128, true) : TB_BWD(64, true);
   else e = (D == 128) ? TB_BWD(128, false) : TB_BWD(64, false);
 #undef TB_BWD

@@ -1,25 +1,21 @@
-// FlashAttention forward on tcgen05 / TMEM / TMA for sm_100a.
+// FlashAttention forward on wgmma / TMA for sm_90a.
 //
-// One CTA per (128-row query tile, q head, batch/sequence).  Warp roles:
-//   warp 0    : TMA producer  -- Q once, then separate rings of K (3 stages) and V (2 stages) tiles (3-D tensor maps over
-//               [tokens, heads, D], SWIZZLE_128B boxes of 64 x 1 x 128, so strided q/k/v views of a fused QKV
-//               activation are read in place)
-//   warp 1    : MMA issuer    -- S = Q K^T (UMMA 128x128xD, K-major/K-major) into a double-buffered TMEM S tile,
-//               O += P V (UMMA 128xDx128, P K-major from smem, V MN-major) into a TMEM O accumulator
-//   warp 2    : TMEM allocator
-//   warps 4-7 : softmax       -- thread i owns query row i (TMEM lane i): tcgen05.ld the S row, scale/mask, online
-//               max/sum in fp32 with exp2, write P as bf16 into 128B-swizzled smem, lazily rescale O in TMEM only
-//               when the running max moved by more than 2^8 (exact: P and the row sum use the same stale max)
-// S(j+1) is issued before P V(j), so the tensor pipe computes the next score tile while the softmax warps work.
+// One CTA per (128-row query tile, q head, batch/sequence), three warpgroups:
+//   warp 0     : TMA producer -- Q once, then 2-stage rings of K and V tiles (3-D tensor maps over [tokens, heads, D],
+//                SWIZZLE_128B boxes of 64 x 1 x 128, so strided q/k/v views of a fused QKV activation are read in place)
+//   warps 4-11 : two MMA warpgroups, 64 query rows each.  Per key tile: S = Q K^T (wgmma m64n128k16, both operands from
+//                shared memory, fp32 scores in registers), scale / mask / online softmax with exp2 (a row lives in the
+//                four lanes of a quad), P converted in registers to the A operand of O += P V (V read MN-major from
+//                shared memory).  The two warpgroups are not synchronised with each other, so one runs its softmax
+//                while the other one occupies the tensor cores.
 // Masking: causal (bottom-right aligned), sliding window (left, right), per-sequence lengths (cu_seqlens) and the
 // ragged tail; GQA by mapping q head h to kv head h / (Hq / Hk).
 //
 // Reference parity: torch_xla custom calls / flash-attn FA2 kernels used by reference torchacc/ops/flash_attn.py
 // (mma.sync, sm80-class); SURVEY 2.4a rows "FA2 forward (fixed)", "FA2 varlen".
 #include <math.h>
+#include <stdio.h>
 #include <stdlib.h>
-
-#include <type_traits>
 
 #include "../common/ptx.cuh"
 #include "../common/tensormap.h"
@@ -30,10 +26,8 @@ namespace tb {
 
 constexpr int kBM = 128;  // query rows per CTA
 constexpr int kBN = 128;  // keys per tile
-constexpr int kKStages = 3;   // K is needed one tile earlier than V (S(t+1) is issued before P V(t)): deeper ring
-constexpr int kVStages = 2;
-constexpr int kFwdThreads = 384;  // 4 control warps + 2 softmax warpgroups (64 key columns each)
-constexpr float kRescaleThreshold = 8.0f;  // log2 domain
+constexpr int kKVStages = 2;
+constexpr int kFwdThreads = 384;  // producer warpgroup + 2 MMA warpgroups
 
 struct FwdArgs {
   uint16_t* o;                 // bf16 or fp16 (kernel template)
@@ -56,28 +50,19 @@ struct FwdArgs {
   float* acc;
   int acc_init;
   DropoutParams drop;   // used by the kDrop instantiations only
-  long long* trace;   // optional [64 tiles][16 slots] clock64 stamps of the first CTA (debug / profiling)
+  long long* trace;     // optional [64 tiles][16 slots] clock64 stamps of the first CTA (debug / profiling)
 };
-
-#define TB_FTRACE(slot)                                                                            \
-  do {                                                                                             \
-    if (args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && t < 64)  \
-      args.trace[t * 16 + (slot)] = clock64();                                                     \
-  } while (0)
 
 template <int D>
 struct FwdSmem {
   static constexpr int kChunks = D / 64;
   static constexpr int kQBytes = kBM * D * 2;
   static constexpr int kKBytes = kBN * D * 2;
-  static constexpr int kPBytes = kBM * kBN * 2;
   static constexpr int kQ = 0;
   static constexpr int kK = kQ + kQBytes;
-  static constexpr int kV = kK + kKStages * kKBytes;
-  static constexpr int kP = kV + kVStages * kKBytes;
-  static constexpr int kBar = kP + kPBytes;
-  static constexpr int kXchg = kBar + 256;              // row max / row sum exchange between the two softmax groups
-  static constexpr int kTotal = kXchg + 2 * kBM * 4 + 1024;
+  static constexpr int kV = kK + kKVStages * kKBytes;
+  static constexpr int kBar = kV + kKVStages * kKBytes;
+  static constexpr int kTotal = kBar + 256 + 1024;
 };
 
 // visible key range [lo, hi] for query row `row` (0-based inside its sequence)
@@ -95,9 +80,6 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
                  const __grid_constant__ CUtensorMap tmap_v, const FwdArgs args) {
   using S = FwdSmem<D>;
   constexpr int kChunks = S::kChunks;
-  constexpr uint32_t kIdescS = make_idesc_f16(kBM, kBN, Major::K, Major::K, kBf16);
-  constexpr uint32_t kIdescO = make_idesc_f16(kBM, D, Major::K, Major::MN, kBf16);
-  constexpr uint32_t kTmemS0 = 0, kTmemO = 2 * kBN;
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const uint32_t lane = lane_id();
@@ -142,19 +124,13 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = base + S::kQ, sK = base + S::kK, sV = base + S::kV, sP = base + S::kP;
+  const uint32_t sQ = base + S::kQ, sK = base + S::kK, sV = base + S::kV;
   const uint32_t bar = base + S::kBar;
   const uint32_t q_full = bar;
   auto k_full = [&](int s) { return bar + 8u * (1 + s); };
-  auto k_empty = [&](int s) { return bar + 8u * (1 + kKStages + s); };
-  auto v_full = [&](int s) { return bar + 8u * (1 + 2 * kKStages + s); };
-  auto v_empty = [&](int s) { return bar + 8u * (1 + 2 * kKStages + kVStages + s); };
-  constexpr int kB0 = 1 + 2 * kKStages + 2 * kVStages;
-  auto s_full = [&](int i) { return bar + 8u * (kB0 + i); };
-  auto s_free = [&](int i) { return bar + 8u * (kB0 + 2 + i); };
-  const uint32_t p_ready = bar + 8u * (kB0 + 4);
-  const uint32_t o_done = bar + 8u * (kB0 + 5);
-  const uint32_t tmem_slot = bar + 8u * (kB0 + 6);
+  auto k_empty = [&](int s) { return bar + 8u * (1 + kKVStages + s); };
+  auto v_full = [&](int s) { return bar + 8u * (1 + 2 * kKVStages + s); };
+  auto v_empty = [&](int s) { return bar + 8u * (1 + 3 * kKVStages + s); };
 
   if (warp_idx == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_q);
@@ -163,700 +139,205 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   }
   if (warp_idx == 1 && lane == 0) {
     mbar_init(q_full, 1);
-    for (int s = 0; s < kKStages; ++s) {
+    for (int s = 0; s < kKVStages; ++s) {
       mbar_init(k_full(s), 1);
-      mbar_init(k_empty(s), 1);
-    }
-    for (int s = 0; s < kVStages; ++s) {
       mbar_init(v_full(s), 1);
-      mbar_init(v_empty(s), 1);
+      mbar_init(k_empty(s), 2);   // one arrival per MMA warpgroup
+      mbar_init(v_empty(s), 2);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(s_full(i), 1);
-      mbar_init(s_free(i), 8);
-    }
-    mbar_init(p_ready, 8);
-    mbar_init(o_done, 1);
     fence_mbar_init();
   }
-  if (warp_idx == 2) tmem_alloc<1>(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp_idx == 0) {
+  if (warp_idx < 4) {
+    setmaxnreg_dec<40>();
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    if (warp_idx == 0 && lane == 0) {
       mbar_arrive_expect_tx(q_full, S::kQBytes);
 #pragma unroll
       for (int c = 0; c < kChunks; ++c) tma_load_3d(sQ + c * 16384, &tmap_q, q_full, c * 64, h, q_start + m0);
-      // K runs ahead of V: issue K(t + 1) before V(t) so the next score tile is never starved
-      auto load_k = [&](int t) {
-        const int s = t % kKStages;
-        mbar_wait(k_empty(s), ((t / kKStages) & 1) ^ 1);
+      for (int t = 0; t < n_tiles; ++t) {
+        const int s = t % kKVStages;
+        const uint32_t ph = ((t / kKVStages) & 1) ^ 1;
+        const int tok = k_start + (j_lo + t) * kBN;
+        mbar_wait(k_empty(s), ph);
         mbar_arrive_expect_tx(k_full(s), S::kKBytes);
 #pragma unroll
-        for (int c = 0; c < kChunks; ++c)
-          tma_load_3d(sK + s * S::kKBytes + c * 16384, &tmap_k, k_full(s), c * 64, hk, k_start + (j_lo + t) * kBN);
-      };
-      auto load_v = [&](int t) {
-        const int s = t % kVStages;
-        mbar_wait(v_empty(s), ((t / kVStages) & 1) ^ 1);
+        for (int c = 0; c < kChunks; ++c) tma_load_3d(sK + s * S::kKBytes + c * 16384, &tmap_k, k_full(s), c * 64, hk, tok);
+        mbar_wait(v_empty(s), ph);
         mbar_arrive_expect_tx(v_full(s), S::kKBytes);
 #pragma unroll
-        for (int c = 0; c < kChunks; ++c)
-          tma_load_3d(sV + s * S::kKBytes + c * 16384, &tmap_v, v_full(s), c * 64, hk, k_start + (j_lo + t) * kBN);
-      };
-      load_k(0);
-      for (int t = 0; t < n_tiles; ++t) {
-        if (t + 1 < n_tiles) load_k(t + 1);
-        load_v(t);
+        for (int c = 0; c < kChunks; ++c) tma_load_3d(sV + s * S::kKBytes + c * 16384, &tmap_v, v_full(s), c * 64, hk, tok);
       }
     }
-  } else if (warp_idx == 1) {
-    // ================================ MMA issuer ================================
-    if (lane == 0) {
-      auto issue_s = [&](int t) {
-        const int s = t % kKStages;
-        const uint32_t kb = sK + s * S::kKBytes;
-        const uint32_t dst = tmem_base + kTmemS0 + (t & 1) * kBN;
+    return;
+  }
+
+  // ================================ MMA + softmax + epilogue ================================
+  setmaxnreg_inc<232>();
+  const int wg = (warp_idx >> 2) - 1;
+  const uint32_t quad = lane & 3;
+  const int r0 = wg * 64 + (warp_idx & 3) * 16 + (int)(lane >> 2);   // this thread's rows inside the tile: r0, r0 + 8
+  const bool elected = (threadIdx.x & 127) == 0;
+  const bool tracing = args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
+  int lo[2], hi[2], pos_q[2];
+  uint32_t drop_row[2] = {0u, 0u};
+  float lse_prev[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint64_t da = desc_kmajor_sw128(sQ + (kk / 4) * 16384, kk % 4);
-          const uint64_t db = desc_kmajor_sw128(kb + (kk / 4) * 16384, kk % 4);
-          umma_ss_f16<1>(dst, da, db, kIdescS, kk != 0);
-        }
-        umma_commit(k_empty(s));       // K tile is free as soon as the score MMAs retire
-        umma_commit(s_full(t & 1));
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(k_full(0), 0);
-      tc_fence_after();
-      issue_s(0);
-      for (int t = 0; t < n_tiles; ++t) {
-        if (t + 1 < n_tiles) {
-          const int s1 = (t + 1) % kKStages;
-          mbar_wait(k_full(s1), ((t + 1) / kKStages) & 1);
-          mbar_wait(s_free((t + 1) & 1), (((t + 1) >> 1) & 1) ^ 1);
-          tc_fence_after();
-          issue_s(t + 1);
-          TB_FTRACE(0);
-        }
-        const int s = t % kVStages;
-        mbar_wait(v_full(s), (t / kVStages) & 1);
-        mbar_wait(p_ready, t & 1);
-        tc_fence_after();
-        TB_FTRACE(1);
-        const uint32_t vb = sV + s * S::kKBytes;
+  for (int i = 0; i < 2; ++i) {
+    const int row = min(m0 + r0 + 8 * i, q_len - 1);
+    key_bounds(row, q_len, k_len, args.causal, args.wl, args.wr, lo[i], hi[i]);
+    pos_q[i] = row + (k_len - q_len);
+    if constexpr (kDrop)
+      drop_row[i] = drop_row_part(drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)), (uint32_t)(m0 + r0 + 8 * i));
+    // running LSE of the previous blocks: read before the epilogue overwrites it
+    if (merging && !args.acc_init && m0 + r0 + 8 * i < q_len)
+      lse_prev[i] = args.lse[(long long)h * args.Tq + q_start + m0 + r0 + 8 * i];
+  }
+  // ALiBi: bias -slope * |query position - key| is folded into the scores (log2 units); the softmax then runs with
+  // scale 1
+  const bool has_alibi = args.alibi != nullptr;
+  const float slope_l2 = has_alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
+  const float sl2 = has_alibi ? 1.f : args.scale_log2;
+
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float oacc[D / 2];
+  mbar_wait(q_full, 0);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int s = t % kKVStages;
+    const uint32_t ph = (t / kKVStages) & 1;
+    const int n0 = (j_lo + t) * kBN;
+    if (tracing && t < 64) args.trace[t * 16 + 0] = clock64();
+    // ---- S = Q K^T ----
+    float sacc[kBN / 2];
+    mbar_wait(k_full(s), ph);
+    wgmma_fence_acc(sacc);
+    wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < kBN / 16; ++kk) {
-          const uint64_t da = desc_kmajor_sw128(sP + (kk / 4) * 16384, kk % 4);
-          const uint64_t db = desc_mnmajor_sw128(vb, kk, 16384);
-          umma_ss_f16<1>(tmem_base + kTmemO, da, db, kIdescO, (t | kk) != 0);
+    for (int kk = 0; kk < D / 16; ++kk)
+      wgmma_ss<kBN, kBf16, 0, 0>(sacc, desc_kmajor_sw128(sQ + (kk / 4) * 16384 + wg * 8192, kk % 4),
+                                 desc_kmajor_sw128(sK + s * S::kKBytes + (kk / 4) * 16384, kk % 4), kk != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(sacc);
+    if (elected) mbar_arrive(k_empty(s));
+    if (tracing && t < 64) args.trace[t * 16 + 1] = clock64();
+
+    // ---- scale / mask / online softmax ----
+    const bool interior = !has_alibi && n0 >= lo[0] && n0 >= lo[1] && n0 + kBN - 1 <= hi[0] && n0 + kBN - 1 <= hi[1];
+    if (!__all_sync(0xffffffffu, interior)) {
+#pragma unroll
+      for (int j = 0; j < kBN / 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int i = e >> 1;
+          const int kidx = n0 + 8 * j + 2 * (int)quad + (e & 1);
+          float v = sacc[4 * j + e];
+          if (has_alibi) v = fmaf(v, args.scale_log2, -slope_l2 * fabsf((float)(pos_q[i] - kidx)));
+          sacc[4 * j + e] = (kidx >= lo[i] && kidx <= hi[i]) ? v : -INFINITY;
         }
-        umma_commit(v_empty(s));
-        umma_commit(o_done);
-      }
     }
-  } else if (warp_idx >= 4) {
-    // ================================ softmax + epilogue ================================
-    // two warpgroups share every row: grp 0 (warps 4-7) owns key columns [0,64) of the tile and O columns
-    // [0,D/2); grp 1 (warps 8-11) owns the other halves.  Row max / row sum are exchanged through smem.
-    const uint32_t q4 = warp_idx & 3;
-    const int grp = (warp_idx - 4) >> 2;
-    const int r = q4 * 32 + lane;        // row inside the tile == TMEM lane
-    const int row = m0 + r;              // row inside the sequence
-    int lo, hi;
-    key_bounds(min(row, q_len - 1), q_len, k_len, args.causal, args.wl, args.wr, lo, hi);
-    const uint32_t lane_off = (q4 * 32u) << 16;
-    float* xchg = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + S::kXchg);
-    float m_used = -INFINITY, l_part = 0.f;
-    // ALiBi: bias -slope * |query position - key| is folded into the scores (log2 units) right after the TMEM load;
-    // the rest of the softmax then runs with scale 1
-    const bool has_alibi = args.alibi != nullptr;
-    const float slope_l2 = has_alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
-    const float sl2 = has_alibi ? 1.f : args.scale_log2;
-    const int pos_q = min(row, q_len - 1) + (k_len - q_len);
-    // running LSE of the previous blocks: read before anybody (group 0 of this row) overwrites it in the epilogue;
-    // the per-tile bar.sync exchanges order this load before that store
-    float lse_prev = -INFINITY;
-    if (merging && !args.acc_init && row < q_len) lse_prev = args.lse[(long long)h * args.Tq + q_start + row];
-    // dropout: P is masked and rescaled on its way to the PV MMA; the softmax statistics use the undropped P
-    const uint32_t drop_row = kDrop ? drop_row_part(drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)),
-                                                    (uint32_t)row) : 0u;
-
-    for (int t = 0; t < n_tiles; ++t) {
-      const int n0 = (j_lo + t) * kBN + grp * 64;   // first key column owned by this thread
-      mbar_wait(s_full(t & 1), (t >> 1) & 1);
-      tc_fence_after();
-      if (warp_idx == 4 && lane == 0) TB_FTRACE(2);
-      uint32_t sv[2][32];
-      const uint32_t s_addr = tmem_base + lane_off + kTmemS0 + (t & 1) * kBN + grp * 64;
-      tmem_ld_32x32b_x32(s_addr, sv[0]);
-      tmem_ld_32x32b_x32(s_addr + 32, sv[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(s_free(t & 1));  // S buffer may be overwritten by S(t+2)
-
-      if (has_alibi) {
+    float alpha[2], mref[2], psum[2] = {0.f, 0.f};
 #pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const float dist = fabsf((float)(pos_q - (n0 + c * 32 + i)));
-            sv[c][i] = __float_as_uint(fmaf(__uint_as_float(sv[c][i]), args.scale_log2, -slope_l2 * dist));
-          }
-      }
-      const bool full_tile = (n0 >= lo) && (n0 + 63 <= hi);
-      const bool warp_full = __all_sync(0xffffffffu, full_tile);
+    for (int i = 0; i < 2; ++i) {
       float mx = -INFINITY;
-      if (warp_full) {
 #pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(sv[c][i]));
-      } else {
-#pragma unroll
-        for (int c = 0; c < 2; ++c)
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int kidx = n0 + c * 32 + i;
-            const float v = (kidx >= lo && kidx <= hi) ? __uint_as_float(sv[c][i]) : -INFINITY;
-            sv[c][i] = __float_as_uint(v);
-            mx = fmaxf(mx, v);
-          }
-      }
-      // combine the row max of the two column halves
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // previous tile's exchange reads are done
-      xchg[grp * kBM + r] = mx;
-      asm volatile("bar.sync 1, 256;" ::: "memory");
-      mx = fmaxf(mx, xchg[(grp ^ 1) * kBM + r]);
-      if (warp_idx == 4 && lane == 0) TB_FTRACE(3);
-      const float m_new = fmaxf(m_used, mx * sl2);
-      // lazy rescale: only move the reference max when it grew by more than the threshold
-      float alpha = 1.f;
-      bool rescale = false;
-      if (m_new > m_used + kRescaleThreshold || m_used == -INFINITY) {
-        if (m_new != -INFINITY) {
-          alpha = (m_used == -INFINITY) ? 0.f : fast_exp2(m_used - m_new);
-          rescale = (m_used != -INFINITY);
-          m_used = m_new;
-        }
-      }
-      const float mref = (m_used == -INFINITY) ? 0.f : m_used;
-      float psum = 0.f;
-      uint32_t pk[2][16];
-#pragma unroll
-      for (int c = 0; c < 2; ++c)
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          float p0 = fast_exp2(fmaf(__uint_as_float(sv[c][2 * i]), sl2, -mref));
-          float p1 = fast_exp2(fmaf(__uint_as_float(sv[c][2 * i + 1]), sl2, -mref));
-          psum += p0 + p1;
-          if constexpr (kDrop) {
-            const uint32_t k0 = (uint32_t)(n0 + c * 32 + 2 * i);
-            p0 = drop_keep(drop_row, drop_key_part(args.drop.seed_hi, k0), args.drop.thresh24) ? p0 * args.drop.rp : 0.f;
-            p1 = drop_keep(drop_row, drop_key_part(args.drop.seed_hi, k0 + 1), args.drop.thresh24) ? p1 * args.drop.rp
-                                                                                                 : 0.f;
-          }
-          pk[c][i] = pack_h2<kBf16>(p0, p1);
-        }
-      l_part = l_part * alpha + psum;
-      if (warp_idx == 4 && lane == 0) TB_FTRACE(4);
-
-      // P buffer and O accumulator are free once P V(t-1) retired
-      if (t > 0) {
-        mbar_wait(o_done, (t - 1) & 1);
-        tc_fence_after();
-      }
-      if (warp_idx == 4 && lane == 0) TB_FTRACE(5);
-      // P -> smem, K-major SWIZZLE_128B: this group's 64 columns form one 16 KB chunk; 16-byte unit u of row r
-      // lives at unit (u ^ (r & 7))
-      const uint32_t chunk_base = sP + grp * 16384 + r * 128;
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const uint32_t unit = (uint32_t)(c * 4 + u) ^ (uint32_t)(r & 7);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(chunk_base + unit * 16), "r"(pk[c][4 * u]),
-                       "r"(pk[c][4 * u + 1]), "r"(pk[c][4 * u + 2]), "r"(pk[c][4 * u + 3])
-                       : "memory");
-        }
-      }
-      if (t > 0 && __any_sync(0xffffffffu, rescale)) {
-#pragma unroll
-        for (int c = 0; c < D / 64; ++c) {
-          const uint32_t o_addr = tmem_base + lane_off + kTmemO + grp * (D / 2) + c * 32;
-          uint32_t ov[32];
-          tmem_ld_32x32b_x32(o_addr, ov);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-          tmem_st_32x32b_x32(o_addr, ov);
-        }
-        tmem_st_wait();
-      }
-      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready);
-      if (warp_idx == 4 && lane == 0) TB_FTRACE(6);
+      for (int j = 0; j < kBN / 8; ++j) mx = fmaxf(mx, fmaxf(sacc[4 * j + 2 * i], sacc[4 * j + 2 * i + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m_run[i], mx * sl2);
+      alpha[i] = (m_run[i] == -INFINITY) ? 0.f : fast_exp2(m_run[i] - m_new);
+      m_run[i] = m_new;
+      mref[i] = (m_new == -INFINITY) ? 0.f : m_new;
     }
-
-    // ---- epilogue: O / l -> bf16, LSE ----
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    xchg[grp * kBM + r] = l_part;
-    asm volatile("bar.sync 1, 256;" ::: "memory");
-    const float l_run = l_part + xchg[(grp ^ 1) * kBM + r];
-    mbar_wait(o_done, (n_tiles - 1) & 1);
-    tc_fence_after();
-    const float inv_l = (l_run > 0.f) ? (1.f / l_run) : 0.f;
-    const bool valid = row < q_len;
-    const float lse_blk = (l_run > 0.f) ? (m_used + log2f(l_run)) * 0.6931471805599453f : -INFINITY;
-    uint16_t* op = args.o + (long long)(q_start + row) * args.o_ts + (long long)h * D + grp * (D / 2);
-    if (!merging) {
+    // P = exp2(score - m) (masked entries are -inf -> 0), packed straight into the A fragments of the P V MMAs;
+    // dropout masks and rescales P on its way to the MMA, the row sums use the undropped P
+    uint32_t pfrag[kBN / 16][4];
 #pragma unroll
-      for (int c = 0; c < D / 64; ++c) {
-        uint32_t ov[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + kTmemO + grp * (D / 2) + c * 32, ov);
-        tmem_ld_wait();
-        if (valid) {
+    for (int j = 0; j < kBN / 8; ++j)
 #pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            uint4 w;
-            w.x = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 0]) * inv_l, __uint_as_float(ov[8 * u + 1]) * inv_l);
-            w.y = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 2]) * inv_l, __uint_as_float(ov[8 * u + 3]) * inv_l);
-            w.z = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 4]) * inv_l, __uint_as_float(ov[8 * u + 5]) * inv_l);
-            w.w = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 6]) * inv_l, __uint_as_float(ov[8 * u + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(op + c * 32 + u * 8) = w;
-          }
+      for (int i = 0; i < 2; ++i) {
+        float p0 = fast_exp2(fmaf(sacc[4 * j + 2 * i], sl2, -mref[i]));
+        float p1 = fast_exp2(fmaf(sacc[4 * j + 2 * i + 1], sl2, -mref[i]));
+        psum[i] += p0 + p1;
+        if constexpr (kDrop) {
+          const uint32_t k0 = (uint32_t)(n0 + 8 * j + 2 * (int)quad);
+          p0 = drop_keep(drop_row[i], drop_key_part(args.drop.seed_hi, k0), args.drop.thresh24) ? p0 * args.drop.rp : 0.f;
+          p1 = drop_keep(drop_row[i], drop_key_part(args.drop.seed_hi, k0 + 1), args.drop.thresh24) ? p1 * args.drop.rp : 0.f;
         }
-        __syncwarp();
+        pfrag[j >> 1][(j & 1) * 2 + i] = pack_h2<kBf16>(p0, p1);
       }
-      if (valid && grp == 0) args.lse[(long long)h * args.Tq + q_start + row] = lse_blk;
-    } else {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) l_run[i] = l_run[i] * alpha[i] + psum[i];
+    if (t > 0) {
+#pragma unroll
+      for (int j = 0; j < D / 8; ++j) {
+        oacc[4 * j + 0] *= alpha[0]; oacc[4 * j + 1] *= alpha[0];
+        oacc[4 * j + 2] *= alpha[1]; oacc[4 * j + 3] *= alpha[1];
+      }
+    }
+    // ---- O += P V ----
+    mbar_wait(v_full(s), ph);
+    wgmma_fence_acc(oacc);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kBN / 16; ++kk)
+      wgmma_rs<D, kBf16, 1>(oacc, pfrag[kk], desc_mnmajor_sw128(sV + s * S::kKBytes, kk, 16384), (t | kk) != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(oacc);
+    if (elected) mbar_arrive(v_empty(s));
+  }
+
+  // ---- epilogue: O / l -> bf16 / fp16, LSE ----
+  const bool vec_o = (args.o_ts % 8 == 0) && (reinterpret_cast<uintptr_t>(args.o) % 16 == 0);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float l = l_run[i];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const int row = m0 + r0 + 8 * i;
+    const bool valid = row < q_len;
+    const float inv_l = (l > 0.f) ? (1.f / l) : 0.f;
+    const float lse_blk = (l > 0.f) ? (m_run[i] + log2f(l)) * 0.6931471805599453f : -INFINITY;
+    float w_old = 0.f, w_new = inv_l, lse_out = lse_blk;
+    if (merging) {
       // log-sum-exp merge with the running result: out = acc * w_old + (O / l) * w_new
-      const float mx = fmaxf(lse_prev, lse_blk);
-      float w_old = 0.f, w_new = 0.f, lse_out = -INFINITY;
+      const float mx = fmaxf(lse_prev[i], lse_blk);
+      w_new = 0.f;
+      lse_out = -INFINITY;
       if (mx != -INFINITY) {
-        const float e_old = __expf(lse_prev - mx), e_new = __expf(lse_blk - mx);   // exp(-inf) == 0
+        const float e_old = __expf(lse_prev[i] - mx), e_new = __expf(lse_blk - mx);   // exp(-inf) == 0
         const float den = e_old + e_new;
         lse_out = mx + __logf(den);
         w_old = e_old / den;
         w_new = inv_l * e_new / den;
       }
-      float* ap = args.acc + ((long long)(q_start + row) * args.Hq + h) * D + grp * (D / 2);
-      const bool read_acc = !args.acc_init;
-#pragma unroll
-      for (int c = 0; c < D / 64; ++c) {
-        uint32_t ov[32];
-        tmem_ld_32x32b_x32(tmem_base + lane_off + kTmemO + grp * (D / 2) + c * 32, ov);
-        tmem_ld_wait();
-        if (valid) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            float4 a0 = make_float4(0.f, 0.f, 0.f, 0.f), a1 = a0;
-            if (read_acc) {
-              a0 = *reinterpret_cast<const float4*>(ap + c * 32 + u * 8);
-              a1 = *reinterpret_cast<const float4*>(ap + c * 32 + u * 8 + 4);
-            }
-            a0.x = fmaf(a0.x, w_old, __uint_as_float(ov[8 * u + 0]) * w_new);
-            a0.y = fmaf(a0.y, w_old, __uint_as_float(ov[8 * u + 1]) * w_new);
-            a0.z = fmaf(a0.z, w_old, __uint_as_float(ov[8 * u + 2]) * w_new);
-            a0.w = fmaf(a0.w, w_old, __uint_as_float(ov[8 * u + 3]) * w_new);
-            a1.x = fmaf(a1.x, w_old, __uint_as_float(ov[8 * u + 4]) * w_new);
-            a1.y = fmaf(a1.y, w_old, __uint_as_float(ov[8 * u + 5]) * w_new);
-            a1.z = fmaf(a1.z, w_old, __uint_as_float(ov[8 * u + 6]) * w_new);
-            a1.w = fmaf(a1.w, w_old, __uint_as_float(ov[8 * u + 7]) * w_new);
-            *reinterpret_cast<float4*>(ap + c * 32 + u * 8) = a0;
-            *reinterpret_cast<float4*>(ap + c * 32 + u * 8 + 4) = a1;
-            uint4 w;
-            w.x = pack_h2<kBf16>(a0.x, a0.y);
-            w.y = pack_h2<kBf16>(a0.z, a0.w);
-            w.z = pack_h2<kBf16>(a1.x, a1.y);
-            w.w = pack_h2<kBf16>(a1.z, a1.w);
-            *reinterpret_cast<uint4*>(op + c * 32 + u * 8) = w;
-          }
-        }
-        __syncwarp();
-      }
-      if (valid && grp == 0) args.lse[(long long)h * args.Tq + q_start + row] = lse_out;
     }
-  }
-
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
-  }
-}
-
-// =====================================================================================================================
-// Forward v2: TWO 128-row query tiles per CTA, one softmax warpgroup each (thread = whole query row), P handed to the
-// tensor core through TENSOR MEMORY (P overwrites its own score tile as bf16 and is the A operand of O += P V).
-//
-// Why: in the kernel above one query tile is in flight per CTA and its two softmax warpgroups share every row (two
-// bar.sync exchanges per key tile + a generic->async proxy fence for P in shared memory): the tensor pipe waits for a
-// serial softmax chain (ncu: tensor pipe 39 % active, ~3000 cycles per 128x128 tile pair for 1024 cycles of MMA).
-// Here the MMA thread alternates between the two query tiles --
-//     S0(t+1) = Q0 K(t+1)^T | O1 += P1(t) V(t) | S1(t+1) = Q1 K(t+1)^T | O0 += P0(t+1) V(t+1) | ...
-// -- so the tensor pipe works for one tile while the other tile's warpgroup runs its softmax; K and V tiles are loaded once
-// for 256 query rows; the row statistics never leave the owning thread (no exchange, no named barriers in the loop).
-// TMEM (512 columns): S0/P0 [0,128)  S1/P1 [128,256)  O0 [256,256+D)  O1 [256+D,256+2D).  P aliases the front of its score
-// tile: chunk c (scores in columns [32c,32c+32)) is converted and stored to columns [16c,16c+16) after it has been read,
-// and S(t+1) of the same query tile is issued (in order) after the P V MMA that consumes P(t).
-// Not covered (dispatch keeps them on the kernel above): dropout, blockwise merge; short sequences (< 256 rows) also stay
-// there because the second tile would be empty.
-// =====================================================================================================================
-constexpr int kF2KStages = 3;
-constexpr int kFwd2Threads = 384;  // 4 control warps + one softmax warpgroup per query tile (thread = query row)
-constexpr int kF2VStages = 2;
-// TB_F2_UNIFORM_MMA: the whole MMA warp runs the issue loop and one elected lane executes the tcgen05 instructions, so the
-// descriptor arithmetic stays warp-uniform (uniform registers) instead of per-thread registers + R2UR moves per MMA.
-#ifndef TB_F2_UNIFORM_MMA
-#define TB_F2_UNIFORM_MMA 1
-#endif
-
-template <int D>
-struct Fwd2Smem {
-  static constexpr int kChunks = D / 64;
-  static constexpr int kTileBytes = kBM * D * 2;          // one 128-row Q tile == one 128-key K or V tile
-  static constexpr int kQ = 0;
-  static constexpr int kK = kQ + 2 * kTileBytes;
-  static constexpr int kV = kK + kF2KStages * kTileBytes;
-  static constexpr int kBar = kV + kF2VStages * kTileBytes;
-  static constexpr int kTotal = kBar + 256 + 1024;
-};
-
-template <int D, bool kBf16>
-__global__ void __launch_bounds__(kFwd2Threads, 1)
-flash_fwd2_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                  const __grid_constant__ CUtensorMap tmap_v, const FwdArgs args) {
-  using S = Fwd2Smem<D>;
-  constexpr int kChunks = S::kChunks;
-  constexpr uint32_t kIdescS = make_idesc_f16(kBM, kBN, Major::K, Major::K, kBf16);
-  constexpr uint32_t kIdescO = make_idesc_f16(kBM, D, Major::K, Major::MN, kBf16);
-  constexpr uint32_t kTmemS = 0, kTmemO = 2 * kBN;
-
-  const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
-  const uint32_t lane = lane_id();
-  const int b = blockIdx.z, h = blockIdx.y;
-  const int hk = h / (args.Hq / args.Hk);
-  const int tile = args.num_q_tiles - 1 - (int)blockIdx.x;  // heavy (late) causal tiles first
-  const int q_start = args.cu_q ? args.cu_q[b] : b * args.q_bs + args.q_off;
-  const int q_len = args.cu_q ? (args.cu_q[b + 1] - q_start) : args.Sq;
-  const int k_start = args.cu_k ? args.cu_k[b] : b * args.k_bs + args.k_off;
-  const int k_len = args.cu_k ? (args.cu_k[b + 1] - k_start) : args.Sk;
-  const int m0 = tile * (2 * kBM);
-  if (m0 >= q_len) return;
-
-  // key tiles touched by the 256 query rows of this CTA (union over both query tiles)
-  int lo_first, hi_first, lo_last, hi_last;
-  const int last_row = min(m0 + 2 * kBM, q_len) - 1;
-  key_bounds(m0, q_len, k_len, args.causal, args.wl, args.wr, lo_first, hi_first);
-  key_bounds(last_row, q_len, k_len, args.causal, args.wl, args.wr, lo_last, hi_last);
-  const int kmin = lo_first, kmax = hi_last;
-  const int j_lo = kmin / kBN;
-  const int j_hi = (kmax < 0 || kmax < kmin) ? j_lo : (kmax / kBN + 1);
-  const int n_tiles = j_hi - j_lo;
-
-  if (n_tiles <= 0) {  // nothing visible: O = 0, LSE = -inf
-    for (int r = threadIdx.x; r < min(2 * kBM, q_len - m0); r += blockDim.x) {
-      uint16_t* op = args.o + (long long)(q_start + m0 + r) * args.o_ts + (long long)h * D;
-      for (int d = 0; d < D; ++d) op[d] = 0;
-      args.lse[(long long)h * args.Tq + q_start + m0 + r] = -INFINITY;
-    }
-    return;
-  }
-
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t sQ = base + S::kQ, sK = base + S::kK, sV = base + S::kV;
-  const uint32_t bar = base + S::kBar;
-  const uint32_t q_full = bar;
-  auto k_full = [&](int s) { return bar + 8u * (1 + s); };
-  auto k_empty = [&](int s) { return bar + 8u * (1 + kF2KStages + s); };
-  auto v_full = [&](int s) { return bar + 8u * (1 + 2 * kF2KStages + s); };
-  auto v_empty = [&](int s) { return bar + 8u * (1 + 2 * kF2KStages + kF2VStages + s); };
-  constexpr int kB0 = 1 + 2 * kF2KStages + 2 * kF2VStages;
-  auto s_full = [&](int g) { return bar + 8u * (kB0 + g); };        // MMA -> softmax warpgroup g: S_g(t) complete
-  auto p_ready = [&](int g) { return bar + 8u * (kB0 + 2 + g); };   // softmax warpgroup g -> MMA: P_g(t) is in TMEM
-  auto o_done = [&](int g) { return bar + 8u * (kB0 + 4 + g); };    // MMA -> softmax warpgroup g: O_g += P_g(t) V(t) done
-  const uint32_t tmem_slot = bar + 8u * (kB0 + 6);
-
-  if (warp_idx == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  if (warp_idx == 1 && lane == 0) {
-    mbar_init(q_full, 1);
-    for (int s = 0; s < kF2KStages; ++s) {
-      mbar_init(k_full(s), 1);
-      mbar_init(k_empty(s), 1);
-    }
-    for (int s = 0; s < kF2VStages; ++s) {
-      mbar_init(v_full(s), 1);
-      mbar_init(v_empty(s), 1);
-    }
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(s_full(g), 1);
-      mbar_init(p_ready(g), 4);     // one arrival per softmax warp of the group
-      mbar_init(o_done(g), 1);
-    }
-    fence_mbar_init();
-  }
-  if (warp_idx == 2) tmem_alloc<1>(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  // register budget follows the work: the control warpgroup (TMA / MMA / TMEM allocator) gives registers back, the two
-  // softmax warpgroups hold a whole 128-column score row per thread
-  if (warp_idx < 4) {
-  // register budget follows the work (setmaxnreg moves registers inside the CTA: the control warpgroup releases what the
-  // softmax warpgroups gain); each softmax thread holds a whole 128-column score row
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-  if (warp_idx == 0) {
-    // ================================ TMA producer ================================
-    if (lane == 0) {
-      mbar_arrive_expect_tx(q_full, 2 * S::kTileBytes);
-#pragma unroll
-      for (int g = 0; g < 2; ++g)
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c)
-          tma_load_3d(sQ + g * S::kTileBytes + c * 16384, &tmap_q, q_full, c * 64, h, q_start + m0 + g * kBM);
-      auto load_k = [&](int t) {
-        const int s = t % kF2KStages;
-        mbar_wait(k_empty(s), ((t / kF2KStages) & 1) ^ 1);
-        mbar_arrive_expect_tx(k_full(s), S::kTileBytes);
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c)
-          tma_load_3d(sK + s * S::kTileBytes + c * 16384, &tmap_k, k_full(s), c * 64, hk, k_start + (j_lo + t) * kBN);
-      };
-      auto load_v = [&](int t) {
-        const int s = t % kF2VStages;
-        mbar_wait(v_empty(s), ((t / kF2VStages) & 1) ^ 1);
-        mbar_arrive_expect_tx(v_full(s), S::kTileBytes);
-#pragma unroll
-        for (int c = 0; c < kChunks; ++c)
-          tma_load_3d(sV + s * S::kTileBytes + c * 16384, &tmap_v, v_full(s), c * 64, hk, k_start + (j_lo + t) * kBN);
-      };
-      load_k(0);
-      for (int t = 0; t < n_tiles; ++t) {
-        if (t + 1 < n_tiles) load_k(t + 1);
-        load_v(t);
-      }
-    }
-  } else if (warp_idx == 1) {
-    // ================================ MMA issuer ================================
-#if TB_F2_UNIFORM_MMA
-    const bool issuer = elect_one_sync();     // every lane runs the loop (warp-uniform descriptor math), one lane issues
-    {
-#else
-    const bool issuer = true;
-    if (lane == 0) {
-#endif
-      // Descriptors are built once per operand tile and advanced by adding to their 14-bit address field ((bytes >> 4):
-      // +2 per 16-element K step inside a 64-wide chunk, +1024 per 16 KB chunk, +128 per 16 key rows of an MN-major V tile).
-      auto issue_s = [&](int g, int t) {       // S_g = Q_g K(t)^T (overwrites S_g / P_g of the previous key tile)
-        const uint64_t da0 = desc_kmajor_sw128(sQ + g * S::kTileBytes, 0);
-        const uint64_t db0 = desc_kmajor_sw128(sK + (t % kF2KStages) * S::kTileBytes, 0);
-        const uint32_t dst = tmem_base + kTmemS + g * kBN;
-#pragma unroll
-        for (int kk = 0; kk < D / 16; ++kk) {
-          const uint64_t off = (uint64_t)((kk / 4) * 1024 + (kk % 4) * 2);
-          if (issuer) umma_ss_f16<1>(dst, da0 + off, db0 + off, kIdescS, kk != 0);
-        }
-        if (issuer) umma_commit(s_full(g));
-      };
-      auto issue_pv = [&](int g, int t) {      // O_g += P_g(t) V(t), P_g read from tensor memory (16 keys = 8 columns per MMA)
-        const uint64_t dv0 = desc_mnmajor_sw128(sV + (t % kF2VStages) * S::kTileBytes, 0, 16384);
-#pragma unroll
-        for (int kk = 0; kk < kBN / 16; ++kk)
-          if (issuer)
-            umma_ts_f16(tmem_base + kTmemO + g * D, tmem_base + kTmemS + g * kBN + kk * 8, dv0 + (uint64_t)(kk * 128),
-                        kIdescO, (t | kk) != 0);
-        if (issuer) umma_commit(o_done(g));
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(k_full(0), 0);
-      tc_fence_after();
-      issue_s(0, 0);
-      issue_s(1, 0);
-      if (issuer) umma_commit(k_empty(0));
-      for (int t = 0; t < n_tiles; ++t) {
-        const bool more = t + 1 < n_tiles;
-        mbar_wait(v_full(t % kF2VStages), (t / kF2VStages) & 1);
-        mbar_wait(p_ready(0), t & 1);
-        tc_fence_after();
-        issue_pv(0, t);
-        if (more) {
-          mbar_wait(k_full((t + 1) % kF2KStages), ((t + 1) / kF2KStages) & 1);
-          tc_fence_after();
-          issue_s(0, t + 1);
-        }
-        mbar_wait(p_ready(1), t & 1);
-        tc_fence_after();
-        issue_pv(1, t);
-        if (issuer) umma_commit(v_empty(t % kF2VStages));
-        if (more) {
-          issue_s(1, t + 1);
-          if (issuer) umma_commit(k_empty((t + 1) % kF2KStages));
-        }
-      }
-    }
-  }
-  } else {
-    // ====== softmax + epilogue: warpgroup g owns query tile g, thread = query row ======
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
-    const uint32_t q4 = warp_idx & 3;
-    const int g = (warp_idx - 4) >> 2;
-    const int r = q4 * 32 + lane;              // row inside the query tile == TMEM lane
-    const int row = m0 + g * kBM + r;          // row inside the sequence
-    int lo, hi;
-    key_bounds(min(row, q_len - 1), q_len, k_len, args.causal, args.wl, args.wr, lo, hi);
-    const uint32_t lane_off = (q4 * 32u) << 16;
-    const uint32_t s_base = tmem_base + lane_off + kTmemS + g * kBN;
-    const uint32_t o_base = tmem_base + lane_off + kTmemO + g * D;
-    float m_used = -INFINITY, l_run = 0.f;
-    const bool has_alibi = args.alibi != nullptr;
-    const float slope_l2 = has_alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
-    const float sl2 = args.scale_log2;
-    const int pos_q = min(row, q_len - 1) + (k_len - q_len);
-
-    for (int t = 0; t < n_tiles; ++t) {
-      const int n0 = (j_lo + t) * kBN;
-      mbar_wait(s_full(g), t & 1);
-      tc_fence_after();
-      // the whole score row (128 fp32) in registers: four loads in flight, ONE wait (waiting after each 32-column load cost
-      // ~4000 cycles of tcgen05.ld latency per key tile: profiles/attn_fwd2_r2.txt)
-      uint32_t sv[4][32];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) tmem_ld_32x32b_x32(s_base + c * 32, sv[c]);
-      tmem_ld_wait();
-      const bool full_tile = (n0 >= lo) && (n0 + kBN - 1 <= hi);
-      const bool warp_full = __all_sync(0xffffffffu, full_tile) && !has_alibi;
-      // Two complete code paths (interior tiles: no mask code at all; boundary / ALiBi tiles: the mask is recomputed where a
-      // value is used), so the score registers are never conditionally rewritten (that kept a second copy of the row alive).
-      auto score = [&](auto masked, int c, int i) -> float {
-        float v = __uint_as_float(sv[c][i]);
-        if constexpr (decltype(masked)::value) {
-          const int kidx = n0 + c * 32 + i;
-          v *= sl2;
-          if (has_alibi) v -= slope_l2 * fabsf((float)(pos_q - kidx));
-          return (kidx >= lo && kidx <= hi) ? v : -INFINITY;
-        } else {
-          return v;    // raw: the caller folds the scale into its FMA
-        }
-      };
-      auto body = [&](auto masked) {
-        constexpr bool kM = decltype(masked)::value;
-        float mxc[4];   // four independent chains (one 128-long dependent chain was 4.5 % slower)
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          mxc[c] = score(masked, c, 0);
-#pragma unroll
-          for (int i = 1; i < 32; ++i) mxc[c] = fmaxf(mxc[c], score(masked, c, i));
-        }
-        float mx = fmaxf(fmaxf(mxc[0], mxc[1]), fmaxf(mxc[2], mxc[3]));
-        if constexpr (!kM) mx *= sl2;
-        const float m_new = fmaxf(m_used, mx);
-        // lazy rescale: only move the reference max when it grew by more than the threshold
-        float alpha = 1.f;
-        bool rescale = false;
-        if (m_new > m_used + kRescaleThreshold || m_used == -INFINITY) {
-          if (m_new != -INFINITY) {
-            alpha = (m_used == -INFINITY) ? 0.f : fast_exp2(m_used - m_new);
-            rescale = (m_used != -INFINITY);
-            m_used = m_new;
-          }
-        }
-        const float mref = (m_used == -INFINITY) ? 0.f : m_used;
-        // P = exp2(score - m) (masked entries are -inf -> 0), row sum, P -> TMEM aliasing the front of the score tile
-        float psum0 = 0.f, psum1 = 0.f;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            float p0, p1;
-            if constexpr (kM) {
-              p0 = fast_exp2(score(masked, c, 2 * i) - mref);
-              p1 = fast_exp2(score(masked, c, 2 * i + 1) - mref);
-            } else {
-              p0 = fast_exp2(fmaf(score(masked, c, 2 * i), sl2, -mref));
-              p1 = fast_exp2(fmaf(score(masked, c, 2 * i + 1), sl2, -mref));
-            }
-            psum0 += p0;
-            psum1 += p1;
-            pk[i] = pack_h2<kBf16>(p0, p1);
-          }
-          tmem_st_32x32b_x16(s_base + c * 16, pk);
-        }
-        l_run = l_run * alpha + (psum0 + psum1);
-        // O_g may be rescaled here: S_g(t) was issued after O_g += P_g(t-1) V(t-1), so that MMA has retired, and the P V MMA
-        // of this tile starts only after our arrival below (placed after the P stores: the score registers are dead by now)
-        if (t > 0 && __any_sync(0xffffffffu, rescale)) {
-#pragma unroll
-          for (int c = 0; c < D / 32; ++c) {
-            uint32_t ov[32];
-            tmem_ld_32x32b_x32(o_base + c * 32, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) ov[i] = __float_as_uint(__uint_as_float(ov[i]) * alpha);
-            tmem_st_32x32b_x32(o_base + c * 32, ov);
-          }
-        }
-      };
-      if (warp_full) body(std::false_type{}); else body(std::true_type{});
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_ready(g));
-    }
-
-    // ---- epilogue: O_g / l -> bf16/fp16, LSE ----
-    mbar_wait(o_done(g), (n_tiles - 1) & 1);
-    tc_fence_after();
-    const float inv_l = (l_run > 0.f) ? (1.f / l_run) : 0.f;
-    const bool valid = row < q_len;
+    float* ap = merging ? args.acc + ((long long)(q_start + row) * args.Hq + h) * D : nullptr;
     uint16_t* op = args.o + (long long)(q_start + row) * args.o_ts + (long long)h * D;
 #pragma unroll
-    for (int c = 0; c < D / 32; ++c) {
-      uint32_t ov[32];
-      tmem_ld_32x32b_x32(o_base + c * 32, ov);
-      tmem_ld_wait();
-      if (valid) {
+    for (int g = 0; g < D / 32; ++g) {
+      uint32_t x[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          uint4 w;
-          w.x = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 0]) * inv_l, __uint_as_float(ov[8 * u + 1]) * inv_l);
-          w.y = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 2]) * inv_l, __uint_as_float(ov[8 * u + 3]) * inv_l);
-          w.z = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 4]) * inv_l, __uint_as_float(ov[8 * u + 5]) * inv_l);
-          w.w = pack_h2<kBf16>(__uint_as_float(ov[8 * u + 6]) * inv_l, __uint_as_float(ov[8 * u + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(op + c * 32 + u * 8) = w;
+      for (int jj = 0; jj < 4; ++jj) {
+        const int j = 4 * g + jj;
+        float v0 = oacc[4 * j + 2 * i] * w_new, v1 = oacc[4 * j + 2 * i + 1] * w_new;
+        if (merging && valid) {
+          float2* a2 = reinterpret_cast<float2*>(ap + 8 * j + 2 * quad);
+          if (!args.acc_init) {
+            const float2 old = *a2;
+            v0 = fmaf(old.x, w_old, v0);
+            v1 = fmaf(old.y, w_old, v1);
+          }
+          *a2 = make_float2(v0, v1);
         }
+        x[jj] = pack_h2<kBf16>(v0, v1);
       }
-      __syncwarp();
+      quad_transpose(x, lane);
+      if (valid) store_row8(op + 32 * g + 8 * quad, x, 8, vec_o);
     }
-    if (valid)
-      args.lse[(long long)h * args.Tq + q_start + row] =
-          (l_run > 0.f) ? (m_used + log2f(l_run)) * 0.6931471805599453f : -INFINITY;
-  }
-
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
+    if (valid && quad == 0) args.lse[(long long)h * args.Tq + q_start + row] = lse_out;
   }
 }
 
@@ -886,34 +367,6 @@ static cudaError_t launch_fwd(const CUtensorMap& mq, const CUtensorMap& mk, cons
   dim3 grid(a.num_q_tiles, a.Hq, a.B);
   kern<<<grid, kFwdThreads, S::kTotal, stream>>>(mq, mk, mv, a);
   return cudaGetLastError();
-}
-
-template <int D, bool kBf16>
-static cudaError_t launch_fwd2(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, FwdArgs a,
-                               int max_q_len, cudaStream_t stream) {
-  using S = Fwd2Smem<D>;
-  auto kern = flash_fwd2_kernel<D, kBf16>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  a.num_q_tiles = (max_q_len + 2 * kBM - 1) / (2 * kBM);
-  dim3 grid(a.num_q_tiles, a.Hq, a.B);
-  kern<<<grid, kFwd2Threads, S::kTotal, stream>>>(mq, mk, mv, a);
-  return cudaGetLastError();
-}
-
-// 1 = always the one-tile kernel, 2 = the two-tile kernel whenever it applies (default), read once from
-// TORCHACC_B200_ATTN_FWD
-static int fwd_version() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("TORCHACC_B200_ATTN_FWD");
-    v = (e && e[0] == '1') ? 1 : 2;
-  }
-  return v;
 }
 
 cudaError_t flash_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_q,
@@ -972,13 +425,6 @@ cudaError_t flash_attn_fwd_ex(const void* q, const void* k, const void* v, void*
     a.drop.seed_hi = (uint32_t)(view.seed >> 32);
   } else {
     a.drop = DropoutParams{0u, 1.f, 0u, 0u};
-  }
-  // two query tiles per CTA whenever the longest sequence fills both (no dropout / blockwise merge there)
-  if (!drop && acc == nullptr && mq_len >= 2 * kBM && fwd_version() == 2) {
-    if (is_bf16) return (D == 128) ? launch_fwd2<128, true>(mq, mk, mv, a, mq_len, stream)
-                                   : launch_fwd2<64, true>(mq, mk, mv, a, mq_len, stream);
-    return (D == 128) ? launch_fwd2<128, false>(mq, mk, mv, a, mq_len, stream)
-                      : launch_fwd2<64, false>(mq, mk, mv, a, mq_len, stream);
   }
 #define TB_FWD(DD, BF)                                                                  \
   (drop ? launch_fwd<DD, BF, true>(mq, mk, mv, a, mq_len, stream)                       \

@@ -49,8 +49,7 @@ TB_DEVICE uint32_t ld_acquire_sys(const uint32_t* p) {
 // Streaming access for the collectives' bulk traffic.  Loads are strong (relaxed.sys: never served from a stale L1
 // line -- the same addresses are rewritten by other SMs / GPUs every step) and do not allocate in L1; loads and stores
 // carry an L2 evict-first policy.  Without it the ~2 GB a collective streams per layer flushes the operand tiles the
-// concurrently running GEMMs keep L2-resident (their L2 hit rate is 83 % when alone) and GEMMs overlapping a collective
-// ran 2.6-3.4x slower (profiles/step_timeline_n2_*.txt).
+// concurrently running GEMMs keep L2-resident and slows every GEMM that overlaps a collective.
 TB_DEVICE uint64_t l2_evict_first_policy() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -108,10 +107,10 @@ TB_DEVICE void barrier_exit(const Pads& pads, int rank, int world, int ch, uint3
 // ----------------------------------------------------------------------------------------------------------
 // all-gather (bytes): out + r*bytes <- peer[r] (+ src_off)
 // ----------------------------------------------------------------------------------------------------------
-// Register budget matters here: these kernels run NEXT TO persistent tcgen05 GEMM CTAs (256 threads x 96 registers).
-// At 32 registers x 512 threads a collective CTA takes a quarter of an SM's register file and co-resides with the
-// GEMM; the first version (128 registers: the whole file) kept every SM it touched closed to the GEMM, which then
-// finished only after the collective (profiles/step_timeline_n2_run15.txt: overlapped GEMMs 3.3x slower).
+// Register budget: 32 registers x 512 threads, a quarter of an SM's register file, so four CTAs fit on an SM.  On sm_90a a
+// wgmma GEMM CTA (384 threads, 168 registers each before setmaxnreg) owns the whole register file of its SM, so a
+// collective CTA and a GEMM CTA never share an SM: collectives take SMs from a concurrently running GEMM, which then
+// uses dynamic scheduling (gemm_sched_mode).  How well the two overlap on H100 has not been measured.
 __global__ void __launch_bounds__(512, 4)
 all_gather_kernel(const __grid_constant__ Peers src, const __grid_constant__ Pads pads, uint8_t* __restrict__ out,
                   size_t bytes, int rank, int world, int ch, uint32_t epoch, uint32_t* block_counter) {
@@ -225,14 +224,11 @@ all_to_all_kernel(const __grid_constant__ Peers src, const __grid_constant__ Pad
 }
 
 // ----------------------------------------------------------------------------------------------------------
-// TMA variants (large messages).  Measured on the Llama-3-8B FSDP step: while a 16-byte-load collective streams over
-// NVLink, every concurrently running tcgen05 GEMM is 1.6-3x slower -- independent of how many CTAs the collective
-// uses or whether the GEMM can claim tiles dynamically -- whereas the fused all-gather->GEMM kernel, whose copy
-// clusters move the same bytes with TMA bulk copies, runs at GEMM-only speed.  Long-latency LSU requests to peer
-// memory sit in the SM<->L2 fabric the GEMM's operand traffic uses; bulk-async copies do not.  So large collectives
+// TMA variants (large messages).  Long-latency LSU requests to peer memory sit in the SM<->L2 fabric that a
+// concurrently running GEMM's operand traffic uses; bulk-async copies do not.  So large collectives
 // are driven by ONE thread per CTA issuing 32 KB `cp.async.bulk` transfers  peer HBM -> smem -> local HBM  (or smem ->
 // 256 reducer threads for reduce-scatter).  A CTA keeps (stages-1) x 32 KB in flight, so <= 16 CTAs fill the link;
-// the SMs they occupy (big smem: no co-residency with a GEMM CTA) are simply skipped by the GEMM's dynamic scheduler.
+// the SMs they occupy (no co-residency with a GEMM CTA) receive no tiles from the GEMM's dynamic schedule.
 // ----------------------------------------------------------------------------------------------------------
 constexpr uint32_t kTmaChunk = 32768;
 constexpr int kTmaStages = 6;
@@ -418,11 +414,10 @@ static int grid_for(size_t bytes, int num_sms) {
   return (int)blocks;
 }
 
-// The collectives run concurrently with persistent tcgen05 GEMM CTAs that need the maximum shared-memory carve-out
-// (~199 KB).  An SM cannot host CTAs of two kernels with different L1/shared carve-outs: with the default (L1-heavy)
-// configuration every SM holding a collective CTA was closed to the GEMM until the collective finished, and GEMMs
-// overlapping a collective ran 3.3x slower (profiles/step_timeline_n2_run15.txt).  Asking for the max-shared
-// carve-out makes both kernels co-resident.
+// The collectives run concurrently with wgmma GEMM CTAs that need the maximum shared-memory carve-out (~199 KB).
+// An SM cannot host CTAs of two kernels with different L1/shared carve-outs, and changing the carve-out of an SM waits
+// for it to drain: asking for the max-shared carve-out here lets an SM pass from a collective CTA to a GEMM CTA (and
+// back) without that reconfiguration.
 template <typename K>
 static void prefer_max_smem_carveout(K kernel) {
   cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
@@ -452,16 +447,14 @@ static int env_int(const char* name, int dflt) {
   const int n = e ? atoi(e) : dflt;
   return n > 0 ? n : dflt;
 }
-// reduce-scatter: CTAs with a 192 KB staging ring (they own their SM; the GEMM's dynamic scheduler skips them)
+// reduce-scatter: CTAs with a 192 KB staging ring (they own their SM)
 static int rs_ctas() {
   static int v = env_int("TORCHACC_B200_COMM_RS_CTAS", 16);
   return v;
 }
-// copy kernels (all-gather / all-to-all): many one-warp CTAs with a SMALL ring (3 x 8 KB) that fits next to a GEMM
-// CTA (199 KB) on the same SM.  A CTA's bulk copies from peer memory do not pipeline deeper than ~32 KB, so
-// bandwidth comes from the number of SMs driving TMA, not from ring depth.  Measured at 2 GPUs
-// (profiles/overlap_geometry_n2_run27.txt): 120 x (3 x 8 KB) -> 457 GB/s with the GEMM 1.08x slower;
-// 16 x (6 x 32 KB) -> 336 GB/s / 1.10x; 32 x (6 x 32 KB) -> 425 GB/s / 1.24x.
+// copy kernels (all-gather / all-to-all): many one-warp CTAs with a small ring (3 x 8 KB).  A CTA's bulk copies from
+// peer memory do not pipeline deeper than ~32 KB, so bandwidth comes from the number of SMs driving TMA, not from ring
+// depth.  The CTA count was chosen on another GPU and has not been re-derived for the 132 SMs of an H100.
 static int tma_ctas() {
   static int v = env_int("TORCHACC_B200_COMM_TMA_CTAS", 120);
   return v;

@@ -1,12 +1,14 @@
-// Thin inline-PTX layer for sm_100a: mbarrier, TMA, tcgen05 (MMA / TMEM), cluster helpers.
+// Thin inline-PTX layer for sm_90a: mbarrier, TMA, cluster helpers (the warpgroup MMA wrappers are in wgmma.cuh).
 // Everything here is a direct wrapper of one PTX instruction so kernels read like the
-// hardware protocol they implement.  Compile with -gencode arch=compute_100a,code=sm_100a.
+// hardware protocol they implement.  Compile with -gencode arch=compute_90a,code=sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+
+#include "wgmma.cuh"
 
 namespace tb {
 
@@ -99,7 +101,7 @@ TB_DEVICE void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 // Low-duty wait for side roles (copy engines): back off between polls so the spinning warp does not compete with the
-// MMA / epilogue warps of the same SM sub-partition for issue slots (and power) while a transfer is in flight.
+// MMA warps of the same SM sub-partition for issue slots (and power) while a transfer is in flight.
 TB_DEVICE void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) __nanosleep(128);
 }
@@ -140,16 +142,6 @@ TB_DEVICE void tma_load_2d(uint32_t smem_dst, const void* desc, uint32_t bar, in
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
       " [%0], [%1, {%3, %4}], [%2], %5;"
       ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(desc)), "r"(bar), "r"(c0), "r"(c1), "l"(hint)
-      : "memory");
-}
-// 2-CTA flavour: bytes are credited to the mbarrier of the leader (even) CTA of the pair.
-TB_DEVICE void tma_load_2d_2sm(uint32_t smem_dst, const void* desc, uint32_t bar, int32_t c0, int32_t c1,
-                               uint64_t hint = kEvictNormal) {
-  uint32_t leader_bar = bar & 0xFEFFFFFFu;
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_dst), "l"(reinterpret_cast<uint64_t>(desc)), "r"(leader_bar), "r"(c0), "r"(c1), "l"(hint)
       : "memory");
 }
 TB_DEVICE void tma_load_3d(uint32_t smem_dst, const void* desc, uint32_t bar, int32_t c0, int32_t c1, int32_t c2,
@@ -199,7 +191,7 @@ TB_DEVICE void bulk_store(void* gdst, uint32_t smem_src, uint32_t bytes) {
                : "memory");
 }
 // Same with an L2 cache policy (createpolicy / kEvict* constants): streaming traffic of the collectives must not evict
-// the operand tiles the GEMMs keep L2-resident (round 1: overlapped GEMMs ran 2.6-3.4x slower without evict-first).
+// the operand tiles the GEMMs keep L2-resident.
 TB_DEVICE void bulk_load_hint(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar, uint64_t policy) {
   asm volatile(
       "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
@@ -222,200 +214,40 @@ TB_DEVICE void tma_store_wait() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// Cluster launch control (sm_100): a running cluster cancels a not-yet-launched cluster of the same grid and
-// receives its coordinates -- hardware work stealing for "persistent" kernels launched with one cluster per tile.
-// The 16-byte response lands in shared memory (of every CTA of the cluster with .multicast) and completes 16
-// transaction bytes on the mbarrier at the same offset.
+// Register reallocation between the warpgroups of a CTA (producer warps give registers to the MMA warpgroups)
 // ----------------------------------------------------------------------------------------------
-template <bool kMulticast>
-TB_DEVICE void clc_try_cancel(uint32_t resp_smem, uint32_t bar) {
-  if constexpr (kMulticast) {
-    asm volatile(
-        "clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.multicast::cluster::all.b128 "
-        "[%0], [%1];" ::"r"(resp_smem), "r"(bar)
-        : "memory");
-  } else {
-    asm volatile("clusterlaunchcontrol.try_cancel.async.shared::cta.mbarrier::complete_tx::bytes.b128 [%0], [%1];"
-                 ::"r"(resp_smem), "r"(bar)
-                 : "memory");
-  }
+template <int N>
+TB_DEVICE void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
 }
-// Returns true and the x coordinate of the first CTA of the cancelled cluster, or false if nothing was left to cancel.
-TB_DEVICE bool clc_query(uint32_t resp_smem, uint32_t& first_ctaid_x) {
-  uint32_t valid, x;
-  asm volatile(
-      "{\n"
-      ".reg .pred p1;\n"
-      ".reg .b128 r;\n"
-      "ld.shared.b128 r, [%2];\n"
-      "clusterlaunchcontrol.query_cancel.is_canceled.pred.b128 p1, r;\n"
-      "selp.u32 %1, 1, 0, p1;\n"
-      "mov.u32 %0, 0;\n"
-      "@p1 clusterlaunchcontrol.query_cancel.get_first_ctaid::x.b32.b128 %0, r;\n"
-      "}\n"
-      : "=r"(x), "=r"(valid)
-      : "r"(resp_smem)
-      : "memory");
-  first_ctaid_x = x;
-  return valid != 0;
+template <int N>
+TB_DEVICE void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, MMA, commit, ld/st, fences
-// ----------------------------------------------------------------------------------------------
-template <int kCtaGroup>
-TB_DEVICE void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  } else {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-  }
-}
-template <int kCtaGroup>
-TB_DEVICE void tmem_dealloc(uint32_t tmem_addr, uint32_t ncols) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_addr), "r"(ncols) : "memory");
-  } else {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_addr), "r"(ncols) : "memory");
+// 4 x 4 transpose of 32-bit values inside each quad of lanes: afterwards x[s] of lane t holds what lane s had in x[t].
+// Turns the 4-byte pieces of an MMA accumulator row into 16 contiguous bytes per lane.
+TB_DEVICE void quad_transpose(uint32_t (&x)[4], uint32_t lane) {
+#pragma unroll
+  for (int m = 1; m <= 2; m <<= 1) {
+    const bool up = (lane & m) != 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if (i & m) continue;
+      const uint32_t send = up ? x[i] : x[i | m];
+      const uint32_t got = __shfl_xor_sync(0xffffffffu, send, m);
+      if (up) x[i] = got; else x[i | m] = got;
+    }
   }
 }
 
-TB_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-TB_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc].  Issued by ONE thread.
-template <int kCtaGroup>
-TB_DEVICE void umma_ss_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (kCtaGroup == 1) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+// Stores 8 consecutive 16-bit values (packed in pairs) of one row: one 16-byte store when alignment allows it.
+TB_DEVICE void store_row8(uint16_t* dst, const uint32_t (&x)[4], int cols_left, bool vec_ok) {
+  if (cols_left >= 8 && vec_ok) {
+    *reinterpret_cast<uint4*>(dst) = make_uint4(x[0], x[1], x[2], x[3]);
   } else {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-        : "memory");
+    for (int j = 0; j < 8 && j < cols_left; ++j) dst[j] = (uint16_t)(x[j >> 1] >> (16 * (j & 1)));
   }
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]  (A operand read from tensor memory).
-TB_DEVICE void umma_ts_f16(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// Make an mbarrier track completion of all previously issued tcgen05.mma of this thread.
-TB_DEVICE void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-TB_DEVICE void umma_commit_2sm(uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-      "h"(cta_mask)
-      : "memory");
-}
-
-// TMEM -> registers: warp reads its 32-lane quarter, 32 consecutive fp32 columns per thread.
-TB_DEVICE void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-TB_DEVICE void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-TB_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM
-TB_DEVICE void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]),
-      "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]),
-      "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-TB_DEVICE void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-TB_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts: cute/arch/mma_sm100_desc.hpp in the vendored CUTLASS tree)
-// ----------------------------------------------------------------------------------------------
-enum class Major : uint32_t { K = 0, MN = 1 };
-
-// Instruction descriptor for kind::f16 with bf16/fp16 inputs and fp32 accumulation.
-//   bits [4,6) D format (1=f32) | [7,10) A format (0=f16,1=bf16) | [10,13) B format
-//   bit 15 A major | bit 16 B major | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t m, uint32_t n, Major a_major, Major b_major,
-                                                      bool is_bf16 = true) {
-  return (1u << 4) | ((is_bf16 ? 1u : 0u) << 7) | ((is_bf16 ? 1u : 0u) << 10) |
-         (static_cast<uint32_t>(a_major) << 15) | (static_cast<uint32_t>(b_major) << 16) | ((n >> 3) << 17) |
-         ((m >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, SWIZZLE_128B, version 1 (Blackwell).
-//   [0,14) addr>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2 (SW128)
-TB_DEVICE uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
-  d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;
-  d |= 2ull << 61;
-  return d;
-}
-
-// K-major operand tile [rows][64 bf16] (128 B per row, 8-row swizzle atoms of 1024 B):
-// SBO = 1024 (next 8-row group), LBO unused (1).  Step of UMMA_K=16 elements = +32 B.
-TB_DEVICE uint64_t desc_kmajor_sw128(uint32_t tile_base, uint32_t k16_idx) {
-  return make_smem_desc_sw128(tile_base + k16_idx * 32u, 16u, 1024u);
-}
-// MN-major operand tile stored as [mn/64][k rows][64 bf16]: each 64-wide MN atom is a
-// [BLOCK_K][128 B] box.  LBO = stride between MN atoms, SBO = 1024 (8 k-rows).
-// Step of UMMA_K=16 rows = +2048 B.
-TB_DEVICE uint64_t desc_mnmajor_sw128(uint32_t tile_base, uint32_t k16_idx, uint32_t atom_stride_bytes) {
-  return make_smem_desc_sw128(tile_base + k16_idx * 2048u, atom_stride_bytes, 1024u);
 }
 
 // ----------------------------------------------------------------------------------------------

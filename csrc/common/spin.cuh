@@ -1,4 +1,4 @@
-// Bounded device-side spins on cross-GPU flags (SURVEY 5.3: the reference has no failure detection; round 1 spun forever).
+// Bounded device-side spins on cross-GPU flags (SURVEY 5.3: the reference has no failure detection).
 // A wait that makes no progress for ~60 s prints which rank / channel / epoch it was waiting for and traps: the host sees a
 // CUDA error instead of a hung GPU.
 #pragma once

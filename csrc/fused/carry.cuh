@@ -1,11 +1,11 @@
 // Collectives carried INSIDE compute kernels ("carry jobs").
 //
 // FSDP moves ~0.4 GB over NVLink per decoder layer and direction (parameter all-gather, gradient reduce-scatter).
-// Run as stand-alone kernels on side streams those transfers fight the persistent tcgen05 GEMMs for SMs, L2 and issue
-// slots (round 1: overlapped GEMMs 1.3x slower, N=8 GEMM time 1.17x the single-GPU value).  Here the transfer is a
+// Run as stand-alone kernels on side streams those transfers fight the persistent wgmma GEMMs for SMs, L2 and issue
+// slots.  Here the transfer is a
 // ROLE of the GEMM kernel itself: warp 3 of every GEMM CTA (idle under static tile scheduling) is a copy engine that
-// moves a slice of the pending collective with TMA bulk copies through a small private smem ring while warps 0/1/4-7
-// run the tcgen05 pipeline of the same CTA.  No extra kernel, no extra stream, no SM taken from the GEMM, and the
+// moves a slice of the pending collective with TMA bulk copies through a small private smem ring while warps 0 and 4-11
+// run the wgmma pipeline of the same CTA.  No extra kernel, no extra stream, no SM taken from the GEMM, and the
 // bytes per launch are budgeted from the GEMM's FLOPs so the transfer ends before the mainloop does.
 //
 //   kind 1  all-gather slice : peer shard r  --cp.async.bulk-->  smem  --cp.async.bulk-->  local gathered buffer
@@ -20,7 +20,7 @@
 //           >= its entry epoch before touching peer memory.  The flag is tied to the point where the data becomes
 //           final, not to the launch that happens to carry the first slice: ranks whose byte budgets differ never
 //           wait on each other's scheduling, and a job may be enqueued later than its data is ready (slack against
-//           GPUs that run a phase a few percent slower, see profiles/carry_skew_n2_r2.txt).
+//           GPUs that run a phase a few percent slower).
 //   exit  : the LAST slice, once every CTA of this rank has finished, publishes e into slot [ch][8 + rank] of every
 //           peer ("I am done reading your buffer") and does NOT wait; whoever is about to overwrite a source buffer
 //           waits for those flags first (symm_wait_done, a one-warp kernel).

@@ -35,7 +35,7 @@ long long carry_pending(long long job_id, int queue);
 // Run everything still queued up to and including `job_id` (0 = all) of `queue` as a stand-alone kernel on `stream`.
 cudaError_t carry_flush(long long job_id, int queue, int num_sms, cudaStream_t stream);
 
-// Bytes of NVLink traffic a GEMM carries per FLOP it executes (default 1.2e-4 = ~190 GB/s next to a 1.6 PFLOP/s GEMM, see profiles/carry_n2_r2.txt; TORCHACC_B200_CARRY_BYTES_PER_FLOP).
+// Bytes of NVLink traffic a GEMM carries per FLOP it executes (default 1.2e-4, not re-tuned for H100; TORCHACC_B200_CARRY_BYTES_PER_FLOP).
 double carry_bytes_per_flop(double v);
 
 // One-warp kernel: wait until every rank published `epoch` in the exit slots of `channel` (see carry.cuh).

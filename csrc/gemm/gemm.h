@@ -1,4 +1,4 @@
-// Public (C++) entry points of the tcgen05 GEMM family.  Raw pointers + stream so the kernels build
+// Public (C++) entry points of the wgmma GEMM family.  Raw pointers + stream so the kernels build
 // without any PyTorch headers; csrc/bindings.cpp wraps them as torch ops.
 #pragma once
 #include <cuda_runtime.h>
@@ -6,18 +6,18 @@
 
 namespace tb {
 
-// D[M,N] (+)= A_op[M,K] * B_op[N,K]^T (+ bias).  bf16 (or, with is_fp16, IEEE fp16) inputs, fp32 accumulation in TMEM.
+// D[M,N] (+)= A_op[M,K] * B_op[N,K]^T (+ bias).  bf16 (or, with is_fp16, IEEE fp16) inputs, fp32 accumulation in registers.
 //   a_mn_major == false : A stored [M][K] (row pitch lda);  true : A stored [K][M]
 //   b_mn_major == false : B stored [N][K] (row pitch ldb);  true : B stored [K][N]
 //   out_fp32            : D is float32 instead of bf16
 //   accumulate          : D += result (gradient accumulation)
-//   cluster             : 1 = one CTA per 128x256 tile, 2 = CTA pair per 256x256 tile (cta_group::2)
+//   cluster             : 1 or 2, kept for ABI compatibility: sm_90a has no CTA-pair MMA, every tile is 128x256 on one CTA
 cudaError_t gemm_bf16(const void* A, const void* B, void* D, const void* bias, int M, int N, int K, long long lda,
                       long long ldb, long long ldd, bool a_mn_major, bool b_mn_major, bool out_fp32, bool accumulate,
                       int cluster, int num_sms, cudaStream_t stream, bool is_fp16 = false);
 
-// Tile scheduling of the unfused GEMM: 1 = dynamic (one cluster per tile, claimed with cluster launch control; robust
-// against SMs that are busy with a concurrent kernel), 0 = static striping over a persistent grid.  mode < 0 queries.
+// Grid shape of the unfused GEMM: 0 = "static", a persistent grid striped over the tiles; 1 = "dynamic", a plain grid
+// of one CTA per tile, so that SMs busy with a concurrent kernel simply receive fewer tiles.  mode < 0 queries.
 int gemm_sched_mode(int mode);
 
 // Same with a separate addend: D = A_op * B_op^T (+ bias) + C, C with D's dtype and row pitch ldc (C may alias D).
@@ -41,7 +41,7 @@ cudaError_t ag_gemm_bf16(const uint64_t* peer_a_full, const uint64_t* pad_ptrs, 
                          uint32_t* block_counter, int channel, uint32_t epoch, int comm_clusters, int num_sms,
                          cudaStream_t stream);
 // GEMM -> reduce-scatter, part 1: partial tiles are stored into the owner rank's staging slot [rank] (peer stores)
-// and counted in peer_counters[owner][rank] (4 arrivals per 128-row CTA tile).
+// and counted in peer_counters[owner][rank] (8 arrivals per 128-row CTA tile: one per MMA warp).
 cudaError_t gemm_rs_bf16(const void* A, const void* B, const uint64_t* peer_stage, const uint64_t* peer_counters,
                          const uint64_t* pad_ptrs, int rows_per_rank, int N, int K, long long lda, long long ldb,
                          bool a_mn_major, bool b_mn_major, int rank, int world, int channel, uint32_t epoch,

@@ -1,4 +1,4 @@
-// Persistent, warp-specialised tcgen05 GEMM for sm_100a.
+// Persistent, warp-specialised wgmma GEMM for sm_90a.
 //
 //   D[M,N] (row-major) (+)= A_op[M,K] * B_op[N,K]^T (+ bias[N])
 //
@@ -8,14 +8,13 @@
 //   dgrad    dx = dy W   : A = dy (K-major),  B = W  (MN-major)
 //   wgrad    dW = dy^T x : A = dy (MN-major), B = x  (MN-major)
 //
-// Structure (one CTA per SM, or one CTA *pair* per 2 SMs with cta_group::2):
-//   warp 0   : TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier full/empty)
-//   warp 1   : MMA issuer     (one elected thread; tcgen05.mma kind::f16, fp32 accumulators in TMEM)
-//   warp 2   : TMEM allocator (512 columns = 2 accumulator stages of 128 lanes x 256 columns)
-//   warps 4-7: epilogue       (tcgen05.ld -> registers -> bias/accumulate/cast -> 16B global stores)
-// The accumulator is double-buffered in TMEM so the epilogue of tile i overlaps the mainloop of tile i+1.
-// With kCluster == 2 the pair computes a 256x256 tile: each CTA stages its own 128 rows of A and 128 of the
-// 256 rows of B, halving shared-memory and L2 traffic per FLOP; only the leader CTA issues MMAs.
+// Structure (one CTA of three warpgroups per SM, 128 x 256 output tile):
+//   warp 0     : TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring of 4 stages, mbarrier full/empty)
+//   warp 3     : carried collective (slices of pending FSDP transfers, fused/carry.cuh)
+//   warps 4-11 : two MMA warpgroups, 64 rows each: wgmma.mma_async m64n256k16 with both operands read from shared
+//                memory, fp32 accumulators in registers (128 per thread; the producer warpgroup hands its registers
+//                over with setmaxnreg), then the epilogue (bias / addend / cast, 16-byte stores after a quad transpose)
+// While the MMA warpgroups run the epilogue of tile i, the producer already fills the ring with tile i+1.
 //
 // Reference parity: replaces the cuBLAS GEMMs the reference reaches through nn.Linear
 // (reference torchacc/__init__.py:97-98 forces XLA onto cuBLAS; eager path uses cuBLASLt).
@@ -31,20 +30,21 @@
 
 namespace tb {
 
-constexpr int kBlockMCta = 128;  // accumulator rows per CTA (TMEM lanes)
-constexpr int kBlockN = 256;     // UMMA N
+constexpr int kBlockM = 128;     // accumulator rows per CTA (64 per MMA warpgroup)
+constexpr int kBlockN = 256;     // wgmma N
 constexpr int kBlockK = 64;      // 128 bytes of bf16 = one swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kNumThreads = 256;
+constexpr int kNumThreads = 384;
+constexpr int kCommCtasPerCluster = 2;   // the fused all-gather counts its copy engines in pairs of CTAs
+enum class Major { K, MN };
 constexpr int kGroupM = 8;       // tile rasterisation: sweep 8 row-tiles before moving along N
 
 constexpr int kMaxPeers = 8;
 
 // Fusion of the GEMM with the adjacent tensor-parallel collective over NVLink peer memory.
 //   kFuse == 1 (all-gather -> GEMM): the A operand is the token-gathered activation.  Every rank owns a symmetric
-//     [world*rows, K] buffer and has already written ITS row block; the leading `comm_clusters` clusters of this
+//     [world*rows, K] buffer and has already written ITS row block; the leading 2 * `comm_clusters` CTAs of this
 //     kernel pull the other ranks' row blocks from peer memory into the local buffer and publish one ready counter
-//     per source rank; the GEMM clusters consume M-tiles in shard order (own block first) and their TMA producers
+//     per source rank; the GEMM CTAs consume M-tiles in shard order (own block first) and their TMA producers
 //     spin on the counter of the shard they are about to read.  The transfer of shard r+1 overlaps the MMAs of shard r.
 //   kFuse == 2 (GEMM -> reduce-scatter): output row block d belongs to rank d.  The epilogue stores the bf16 partial
 //     tile straight into rank d's staging slot [my_rank] with peer stores and bumps a per-(dst, src) arrival counter
@@ -59,7 +59,7 @@ struct FuseArgs {
   int rank, world, rows_per_rank, channel;
   uint32_t epoch;                 // monotonically increasing per call on this channel
   uint32_t flag_target;           // kFuse 1: counter value that means "shard complete" for this call
-  int comm_clusters;              // kFuse 1: leading clusters acting as copy engines
+  int comm_clusters;              // kFuse 1: pairs of leading CTAs acting as copy engines
   long long slot_stride;          // kFuse 2: elements between two source slots of a staging buffer
 };
 
@@ -72,15 +72,14 @@ struct GemmArgs {
   long long ldc;   // a different C fuses a residual add into the epilogue (h + x W^T).
   int out_fp32;
   int num_m_tiles, num_n_tiles;
-  // SwiGLU epilogue (gate|up projection, cta_group::2 only): B is W_gu [2F][K]; CTA 0 of a pair stages 128 gate rows,
-  // CTA 1 the matching 128 up rows, so accumulator columns [0,128) / [128,256) are gate / up of the SAME 128 output
-  // columns and the epilogue writes h = silu(g) * u [M][F] directly (and g|u [M][2F] only when the backward needs it).
+  // SwiGLU epilogue (gate|up projection): B is W_gu [2F][K]; a stage holds 128 gate rows followed by the matching 128
+  // up rows, so accumulator columns [0,128) / [128,256) are gate / up of the SAME 128 output columns and the
+  // epilogue writes h = silu(g) * u [M][F] directly (and g|u [M][2F] only when the backward needs it).
   int swiglu;      // 0 / 1
   int swiglu_F;    // F = intermediate size
   void* gu_out;    // optional [M][2F] pre-activation (nullptr: not materialised)
   long long ldgu;
-  int fp16;        // operands, bias and 16-bit outputs are IEEE fp16 instead of bf16 (same tiles, other format bits)
-  int dynamic;     // 1: grid = one cluster per tile, tiles are claimed with cluster-launch-control (see kernel comment)
+  int dynamic;     // 1: grid = one CTA per tile instead of a persistent grid (see gemm_sched_mode)
   FuseArgs fuse;
   CarryArgs carry;  // slices of pending FSDP collectives moved by warp 3 of every CTA while the tiles run (fused/carry.cuh)
 };
@@ -124,10 +123,10 @@ TB_DEVICE void fused_barrier(const FuseArgs& f, bool signal, int slot_base, int 
                      "fused GEMM barrier");
 }
 
-// Copy-engine role of the all-gather -> GEMM kernel (executed by whole clusters).  One thread per CTA drives a ring
+// Copy-engine role of the all-gather -> GEMM kernel (executed by whole CTAs).  One thread per CTA drives a ring
 // of 32 KB TMA bulk copies  peer HBM --NVLink--> smem --> local gathered buffer:  (stages-1) x 32 KB are in flight per
 // CTA, so a handful of CTAs keep the link full (16-byte register loads would need ~100 CTAs for the same bytes in
-// flight).  Shard r is announced to the MMA clusters' TMA producers through flags[r] when all copy CTAs finished it.
+// flight).  Shard r is announced to the GEMM CTAs' TMA producers through flags[r] when all copy CTAs finished it.
 TB_DEVICE void gather_role(const FuseArgs& f, int K, int comm_cta, int num_comm_ctas, uint32_t smem_base,
                            uint32_t bar_base, int num_stages) {
   constexpr uint32_t kChunk = 32768;
@@ -190,13 +189,11 @@ TB_DEVICE void gather_role(const FuseArgs& f, int K, int comm_cta, int num_comm_
   fused_barrier(f, true, 8, threadIdx.x);
 }
 
-template <int kCluster>
 struct GemmSmem {
-  static constexpr int kLoadN = kBlockN / kCluster;
-  static constexpr int kABytes = kBlockMCta * kBlockK * 2;
-  static constexpr int kBBytes = kLoadN * kBlockK * 2;
+  static constexpr int kABytes = kBlockM * kBlockK * 2;
+  static constexpr int kBBytes = kBlockN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (kCluster == 2) ? 6 : 4;
+  static constexpr int kStages = 4;
   static constexpr int kBarrierBytes = 1024;
   static constexpr int kTotal = kStages * kStageBytes + kBarrierBytes + 1024;  // +1024 alignment slack
   static constexpr int kTotalCarry = kTotal + kCarrySmemBytes;                 // + the copy warp's private ring
@@ -224,15 +221,13 @@ __device__ __forceinline__ void tile_coords_sharded(int t, int tiles_m_per_shard
   tn = ln;
 }
 
-template <int kCluster, Major kAMajor, Major kBMajor, int kFuse>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmArgs args) {
-  using S = GemmSmem<kCluster>;
+  using S = GemmSmem;
   constexpr int kStages = S::kStages;
-  constexpr int kLoadN = S::kLoadN;
-  constexpr uint32_t kUmmaM = kBlockMCta * kCluster;
-  constexpr uint32_t kIdesc = make_idesc_f16(kUmmaM, kBlockN, kAMajor, kBMajor, true);
+  constexpr int kTA = (kAMajor == Major::MN) ? 1 : 0, kTB = (kBMajor == Major::MN) ? 1 : 0;
 
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
@@ -240,38 +235,26 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const uint32_t bar_base = smem_base + kStages * S::kStageBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * kStages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * kStages + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kStages + 4);
-  // dynamic tile scheduler (cluster launch control): 16-byte responses + full/empty barriers
-  constexpr int kSched = 4;
-  auto clc_full = [&](int s) { return bar_base + 8u * (2 * kStages + 6 + s); };
-  auto clc_empty = [&](int s) { return bar_base + 8u * (2 * kStages + 6 + kSched + s); };
-  auto clc_resp = [&](int s) { return bar_base + 512u + 16u * s; };
-  constexpr uint32_t kSchedConsumers = 5 * kCluster + 1;   // per CTA: TMA warp + 4 epilogue warps; + the MMA warp
   auto smem_a = [&](int s) { return smem_base + s * S::kStageBytes; };
   auto smem_b = [&](int s) { return smem_base + s * S::kStageBytes + S::kABytes; };
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const uint32_t lane = lane_id();
-  const uint32_t cta_rank = (kCluster == 2) ? cluster_ctarank() : 0u;
-  const bool is_leader = cta_rank == 0;
 
   const int num_tiles = args.num_m_tiles * args.num_n_tiles;
   const int num_k_blocks = (args.K + kBlockK - 1) / kBlockK;
-  int cluster_id = blockIdx.x / kCluster;
-  int num_clusters = gridDim.x / kCluster;
+  int cta = blockIdx.x;
+  int num_ctas = gridDim.x;
   if constexpr (kFuse == 1) {
-    const int cc = args.fuse.comm_clusters;
-    if (cluster_id < cc) {   // copy-engine clusters: no TMEM, no MMA
-      gather_role(args.fuse, args.K, (int)blockIdx.x, cc * kCluster, smem_base, bar_base,
-                  kStages * S::kStageBytes / 32768);
+    const int cc = args.fuse.comm_clusters * kCommCtasPerCluster;
+    if (cta < cc) {   // copy-engine CTAs: no MMA
+      gather_role(args.fuse, args.K, cta, cc, smem_base, bar_base, kStages * S::kStageBytes / 32768);
       return;
     }
-    cluster_id -= cc;
-    num_clusters -= cc;
+    cta -= cc;
+    num_ctas -= cc;
   }
-  const int tiles_m_per_shard = (kFuse != 0) ? args.fuse.rows_per_rank / (kBlockMCta * kCluster) : 0;
+  const int tiles_m_per_shard = (kFuse != 0) ? args.fuse.rows_per_rank / kBlockM : 0;
   // fused tile order: all-gather starts with the local row block; reduce-scatter ends with it (peers first)
   const int first_shard = (kFuse == 1) ? args.fuse.rank : ((kFuse == 2) ? (args.fuse.rank + 1) % args.fuse.world : 0);
   auto coords = [&](int t, int& tm, int& tn, int& shard) {
@@ -290,170 +273,79 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (warp_idx == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 4 * kCluster);  // one arrive per epilogue warp (of both CTAs)
-    }
-    for (int s = 0; s < kSched; ++s) {
-      mbar_init(clc_full(s), 1);
-      mbar_init(clc_empty(s), kSchedConsumers);
+      mbar_init(empty_bar(s), 2);   // one arrival per MMA warpgroup
     }
     fence_mbar_init();
   }
-  if (warp_idx == 2) tmem_alloc<kCluster>(tmem_slot, 512);
-  tc_fence_before();
-  if constexpr (kCluster == 2) cluster_sync(); else __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
+  __syncthreads();
 
-  // ---- tile iteration ----
-  // static : tile = cluster_id, += num_clusters (one resident cluster per SM pair for the whole kernel)
-  // dynamic: the grid has one cluster per tile.  A launched cluster starts with the tile of its own index and then
-  //          claims not-yet-launched clusters through cluster launch control until none is left.  SMs that are busy
-  //          with another kernel (a collective on a side stream) simply join late or never: the remaining clusters
-  //          absorb their tiles instead of the whole GEMM waiting for stragglers.
-  const bool dynamic = (kFuse == 0) && args.dynamic != 0;
-  int sched_it = 0;   // per role thread: position in the response pipeline
-  auto advance = [&](int& tile, bool do_arrive) -> bool {
-    if (!dynamic) {
-      tile += num_clusters;
-      return tile < num_tiles;
-    }
-    const int s = sched_it % kSched;
-    mbar_wait(clc_full(s), (sched_it / kSched) & 1);
-    uint32_t x;
-    const bool valid = clc_query(clc_resp(s), x);
-    fence_proxy_async_smem();   // our read of the response precedes the next asynchronous write of this slot
-    if (do_arrive) {
-      if constexpr (kCluster == 2) mbar_arrive_cluster(mapa_shared(clc_empty(s), 0));
-      else mbar_arrive(clc_empty(s));
-    }
-    ++sched_it;
-    tile = (int)(x / kCluster);
-    return valid;
-  };
-  if (dynamic && warp_idx == 3 && lane == 0) {
-    // ================================ Tile scheduler ================================
-    for (int it = 0;; ++it) {
-      const int s = it % kSched;
-      if (is_leader && it >= kSched) {   // every consumer (of both CTAs) has read the previous response in this slot
-        if constexpr (kCluster == 2) mbar_wait_cluster(clc_empty(s), ((it / kSched) - 1) & 1);
-        else mbar_wait(clc_empty(s), ((it / kSched) - 1) & 1);
-      }
-      mbar_arrive_expect_tx(clc_full(s), 16);       // each CTA arms its own barrier; the response is multicast
-      if (is_leader) clc_try_cancel<kCluster == 2>(clc_resp(s), clc_full(s));
-      mbar_wait(clc_full(s), (it / kSched) & 1);
-      uint32_t x;
-      if (!clc_query(clc_resp(s), x)) break;
-    }
-  }
-
-  if (warp_idx == 0) {
-    // ================================ TMA producer ================================
-    if (lane == 0) {
-      int it = 0;
-      int t = cluster_id;
-      for (bool more = t < num_tiles; more; more = advance(t, true)) {
-        int tm, tn, shard;
-        coords(t, tm, tn, shard);
-        const int m0 = tm * (int)kUmmaM + (int)cta_rank * kBlockMCta;
-        const int n0 = (kFuse == 0 && args.swiglu) ? tn * kLoadN + (int)cta_rank * args.swiglu_F
-                                                   : tn * kBlockN + (int)cta_rank * kLoadN;
-        if constexpr (kFuse == 1) {
-          if (shard != args.fuse.rank) {   // wait until the copy clusters have landed this source rank's rows
-            spin_until_count(args.fuse.flags + shard, args.fuse.flag_target, args.fuse.rank, shard,
-                             "all-gather -> GEMM shard flag");
-            fence_proxy_async_all();       // generic-proxy writes of the copy CTAs -> visible to TMA
+  if (warp_idx < 4) {
+    // the producer warpgroup gives its registers to the two MMA warpgroups (128 accumulator registers per thread)
+    setmaxnreg_dec<56>();
+    if (warp_idx == 0) {
+      // ================================ TMA producer ================================
+      if (lane == 0) {
+        int it = 0;
+        for (int t = cta; t < num_tiles; t += num_ctas) {
+          int tm, tn, shard;
+          coords(t, tm, tn, shard);
+          const int m0 = tm * kBlockM;
+          // SwiGLU: accumulator columns [0,128) are gate rows, [128,256) the matching up rows of W_gu
+          const int n0 = (kFuse == 0 && args.swiglu) ? tn * (kBlockN / 2) : tn * kBlockN;
+          const int n1 = (kFuse == 0 && args.swiglu) ? args.swiglu_F + n0 : n0 + kBlockN / 2;
+          if constexpr (kFuse == 1) {
+            if (shard != args.fuse.rank) {   // wait until the copy CTAs have landed this source rank's rows
+              spin_until_count(args.fuse.flags + shard, args.fuse.flag_target, args.fuse.rank, shard,
+                               "all-gather -> GEMM shard flag");
+              fence_proxy_async_all();       // generic-proxy writes of the copy CTAs -> visible to TMA
+            }
           }
-        }
-        for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait(empty_bar(s), ph ^ 1);
-          if (is_leader) mbar_arrive_expect_tx(full_bar(s), S::kStageBytes * kCluster);
-          const int k0 = kb * kBlockK;
-          auto load = [&](uint32_t dst, const CUtensorMap* map, int c0, int c1) {
-            if constexpr (kCluster == 2) tma_load_2d_2sm(dst, map, full_bar(s), c0, c1);
-            else tma_load_2d(dst, map, full_bar(s), c0, c1);
-          };
-          if constexpr (kAMajor == Major::K) {
-            load(smem_a(s), &tmap_a, k0, m0);
-          } else {
+          for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
+            const int s = it % kStages;
+            mbar_wait(empty_bar(s), ((it / kStages) & 1) ^ 1);
+            mbar_arrive_expect_tx(full_bar(s), S::kStageBytes);
+            const int k0 = kb * kBlockK;
+            if constexpr (kAMajor == Major::K) {
+              tma_load_2d(smem_a(s), &tmap_a, full_bar(s), k0, m0);
+            } else {
 #pragma unroll
-            for (int i = 0; i < kBlockMCta / 64; ++i) load(smem_a(s) + i * 8192, &tmap_a, m0 + i * 64, k0);
-          }
-          if constexpr (kBMajor == Major::K) {
-            load(smem_b(s), &tmap_b, k0, n0);
-          } else {
+              for (int i = 0; i < kBlockM / 64; ++i)
+                tma_load_2d(smem_a(s) + i * 8192, &tmap_a, full_bar(s), m0 + i * 64, k0);
+            }
+            if constexpr (kBMajor == Major::K) {
+              tma_load_2d(smem_b(s), &tmap_b, full_bar(s), k0, n0);
+              tma_load_2d(smem_b(s) + S::kBBytes / 2, &tmap_b, full_bar(s), k0, n1);
+            } else {
 #pragma unroll
-            for (int i = 0; i < kLoadN / 64; ++i) load(smem_b(s) + i * 8192, &tmap_b, n0 + i * 64, k0);
+              for (int i = 0; i < kBlockN / 64; ++i)
+                tma_load_2d(smem_b(s) + i * 8192, &tmap_b, full_bar(s), n0 + i * 64, k0);
+            }
           }
         }
       }
-    }
-  } else if (warp_idx == 1) {
-    // ================================ MMA issuer ================================
-    if (is_leader && lane == 0) {
-      // a/b format bits [7,10) / [10,13): 1 = bf16, 0 = fp16
-      const uint32_t idesc = args.fp16 ? (kIdesc & ~((7u << 7) | (7u << 10))) : kIdesc;
-      int it = 0, lt = 0;
-      int t = cluster_id;
-      for (bool more = t < num_tiles; more; more = advance(t, true), ++lt) {
-        const int as = lt & 1;
-        const uint32_t aph = (lt >> 1) & 1;
-        if constexpr (kCluster == 2) mbar_wait_cluster(tempty_bar(as), aph ^ 1);
-        else mbar_wait(tempty_bar(as), aph ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * kBlockN;
-        for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait(full_bar(s), ph);
-          tc_fence_after();
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = (kAMajor == Major::K) ? desc_kmajor_sw128(smem_a(s), k)
-                                                       : desc_mnmajor_sw128(smem_a(s), k, 8192);
-            const uint64_t db = (kBMajor == Major::K) ? desc_kmajor_sw128(smem_b(s), k)
-                                                       : desc_mnmajor_sw128(smem_b(s), k, 8192);
-            umma_ss_f16<kCluster>(tmem_d, da, db, idesc, (kb | k) != 0);
-          }
-          // Release the smem slot once the MMAs that read it retire.
-          if constexpr (kCluster == 2) umma_commit_2sm(empty_bar(s), 0x3);
-          else umma_commit(empty_bar(s));
+    } else if (warp_idx == 3) {
+      // ================================ Carried collective ================================
+      // Under static scheduling this warp moves this launch's slice of the pending FSDP all-gather / reduce-scatter
+      // (TMA bulk copies through a private 24 KB ring) while the tiles are computed.
+      if constexpr (kFuse == 0) {
+        if (!args.dynamic && args.carry.slice[0].kind != 0) {
+          const uint32_t ring = bar_base + S::kBarrierBytes;
+          carry_role(args.carry, ring, ring + kCarryStages * kCarryStageBytes, (int)blockIdx.x, (int)gridDim.x);
         }
-        if constexpr (kCluster == 2) umma_commit_2sm(tfull_bar(as), 0x3);
-        else umma_commit(tfull_bar(as));
       }
     }
-  } else if (warp_idx == 3) {
-    // ================================ Carried collective ================================
-    // Under static scheduling this warp has no GEMM role: it moves this launch's slice of the pending FSDP
-    // all-gather / reduce-scatter (TMA bulk copies through a private 24 KB ring) while the tiles are computed.
-    if constexpr (kFuse == 0) {
-      if (!dynamic && args.carry.slice[0].kind != 0) {
-        const uint32_t ring = bar_base + S::kBarrierBytes;
-        carry_role(args.carry, ring, ring + kCarryStages * kCarryStageBytes, (int)blockIdx.x, (int)gridDim.x);
-      }
-    }
-  } else if (warp_idx >= 4) {
-    // ================================ Epilogue ================================
-    const uint32_t q = warp_idx & 3;  // TMEM lane quarter this warp may read
-    const bool f16 = args.fp16 != 0;
-    auto unpk = [&](uint32_t u) { return f16 ? unpack_f16x2(u) : unpack_bf16x2(u); };
-    auto pk = [&](float a, float b) { return f16 ? pack_f16x2(a, b) : pack_bf16x2(a, b); };
-    auto ld1 = [&](const __nv_bfloat16* p) {
-      return f16 ? __half2float(*reinterpret_cast<const __half*>(p)) : __bfloat162float(*p);
+  } else {
+    // ================================ MMA + epilogue (two warpgroups, 64 rows each) ================================
+    setmaxnreg_inc<224>();
+    const int wg = (warp_idx >> 2) - 1;              // 0 / 1: rows [64 wg, 64 wg + 64) of the tile
+    const int wq = warp_idx & 3;
+    const uint32_t quad = lane & 3;
+    const int frag_row = wg * 64 + wq * 16 + (int)(lane >> 2);
+    auto pk = [&](float a, float b) { return pack_h2<kBf16>(a, b); };
+    auto ld1 = [&](const uint16_t* p) {
+      return kBf16 ? __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(p))
+                   : __half2float(*reinterpret_cast<const __half*>(p));
     };
-    auto st1 = [&](__nv_bfloat16* p, float v) {
-      if (f16) *reinterpret_cast<__half*>(p) = __float2half_rn(v); else *p = __float2bfloat16(v);
-    };
-    const uint32_t tempty_leader =
-        (kCluster == 2) ? mapa_shared(tempty_bar(0), 0) : tempty_bar(0);  // barrier lives in the leader CTA
-    int lt = 0;
     if constexpr (kFuse == 2) {
       // nobody may write into a peer's staging buffer before that peer finished reducing the previous call
       fused_barrier(args.fuse, blockIdx.x == 0 && warp_idx == 4, 0, (int)lane);
@@ -473,204 +365,179 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
       }
     };
-    int t = cluster_id;
-    for (bool more = t < num_tiles; more; more = advance(t, lane == 0), ++lt) {
+    int it = 0;
+    for (int t = cta; t < num_tiles; t += num_ctas) {
       int tm, tn, shard;
       coords(t, tm, tn, shard);
-      const int as = lt & 1;
-      const uint32_t aph = (lt >> 1) & 1;
-      mbar_wait(tfull_bar(as), aph);
-      tc_fence_after();
-      const long long grow = (long long)tm * kUmmaM + cta_rank * kBlockMCta + q * 32 + lane;
-      const int n0 = tn * kBlockN;
-      const bool row_ok = grow < args.M;
+      float acc[kBlockN / 2];
+      for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
+        const int s = it % kStages;
+        mbar_wait(full_bar(s), (it / kStages) & 1);
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / 16; ++k) {
+          const uint64_t da = (kAMajor == Major::K) ? desc_kmajor_sw128(smem_a(s) + wg * 8192, k)
+                                                     : desc_mnmajor_sw128(smem_a(s) + wg * 8192, k, 8192);
+          const uint64_t db = (kBMajor == Major::K) ? desc_kmajor_sw128(smem_b(s), k)
+                                                     : desc_mnmajor_sw128(smem_b(s), k, 8192);
+          wgmma_ss<kBlockN, kBf16, kTA, kTB>(acc, da, db, (kb | k) != 0);
+        }
+        wgmma_commit();
+        if (kb > 0) {   // the MMAs of the previous K block have retired: hand its smem slot back to the producer
+          wgmma_wait<1>();
+          if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar((it - 1) % kStages));
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar((it - 1) % kStages));
+
+      const long long row0 = (long long)tm * kBlockM + frag_row;   // this thread's rows: row0 and row0 + 8
       if constexpr (kFuse == 2) {
-        // bf16 partial tile -> staging slot [my rank] of the rank that owns this row block (peer stores over NVLink).
-        // The staging layout is block-major: one 2 KB block per (tile, CTA half, lane quarter, 32-column chunk),
-        // inside a block [j][lane][8 columns], so every warp-wide store instruction writes 512 contiguous bytes
-        // (full NVLink packets) instead of 32 scattered 16-byte pieces.  rs_reduce_kernel undoes the permutation.
+        // bf16 partial tile -> staging slot [my rank] of the rank that owns this row block (peer stores over NVLink,
+        // 16 bytes per lane after the quad transpose); slots are row-major [rows_per_rank][N padded to the tile].
         if (shard != cur_shard) {
           flush_arrivals();
           cur_shard = shard;
         }
-        const int tm_local = tm - shard * tiles_m_per_shard;
-        const long long blk0 = ((((long long)tm_local * args.num_n_tiles + tn) * 2 + cta_rank) * 4 + q) * 8;
-        uint4* dbase = reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(args.fuse.peer[shard]) +
-                                                (long long)args.fuse.rank * args.fuse.slot_stride) + blk0 * 128 + lane;
-#pragma unroll 1
-        for (int c = 0; c < kBlockN / 32; ++c) {
-          __syncwarp();
-          uint32_t r[32];
-          tmem_ld_32x32b_x32(tmem_base + ((q * 32u) << 16) + as * kBlockN + c * 32, r);
-          tmem_ld_wait();
-          if (n0 + c * 32 + 32 > args.N) continue;     // (rows are always in range: rows_per_rank % 256 == 0)
-          uint4* d4 = dbase + c * 128;
+        const long long npad = (long long)args.num_n_tiles * kBlockN;
+        uint16_t* slot = reinterpret_cast<uint16_t*>(args.fuse.peer[shard]) + (long long)args.fuse.rank * args.fuse.slot_stride;
+        const long long lrow0 = row0 - (long long)shard * args.fuse.rows_per_rank;
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 o;
-            o.x = pack_bf16x2(__uint_as_float(r[8 * j + 0]), __uint_as_float(r[8 * j + 1]));
-            o.y = pack_bf16x2(__uint_as_float(r[8 * j + 2]), __uint_as_float(r[8 * j + 3]));
-            o.z = pack_bf16x2(__uint_as_float(r[8 * j + 4]), __uint_as_float(r[8 * j + 5]));
-            o.w = pack_bf16x2(__uint_as_float(r[8 * j + 6]), __uint_as_float(r[8 * j + 7]));
-            d4[j * 32] = o;
+        for (int g = 0; g < kBlockN / 32; ++g) {
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            uint32_t x[4];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) x[jj] = pack_bf16x2(acc[4 * (4 * g + jj) + 2 * half], acc[4 * (4 * g + jj) + 2 * half + 1]);
+            quad_transpose(x, lane);
+            const int col = tn * kBlockN + 32 * g + 8 * (int)quad;
+            if (col + 8 <= args.N)
+              *reinterpret_cast<uint4*>(slot + (lrow0 + 8 * half) * npad + col) = make_uint4(x[0], x[1], x[2], x[3]);
           }
         }
         ++pending;
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (kCluster == 2) mbar_arrive_cluster(tempty_leader + 8u * as);
-          else mbar_arrive(tempty_leader + 8u * as);
-        }
         continue;
       }
-      if constexpr (kFuse == 0 && kCluster == 2) {
+      if constexpr (kFuse == 0) {
         if (args.swiglu) {
-          const int oc0 = tn * 128;     // output columns of this tile
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            __syncwarp();
-            uint32_t rg[32], ru[32];
-            tmem_ld_32x32b_x32(tmem_base + ((q * 32u) << 16) + as * kBlockN + c * 32, rg);
-            tmem_ld_32x32b_x32(tmem_base + ((q * 32u) << 16) + as * kBlockN + 128 + c * 32, ru);
-            tmem_ld_wait();
-            const int gcol = oc0 + c * 32;
-            if (!row_ok || gcol >= args.swiglu_F) continue;
-            __nv_bfloat16* hp = reinterpret_cast<__nv_bfloat16*>(args.D) + grow * args.ldd + gcol;
-            uint4* h4 = reinterpret_cast<uint4*>(hp);
-            float hv[32];
+          const bool vec_h = true;   // F % 128 == 0 and the row pitches are multiples of 8 elements (checked on the host)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float g = __uint_as_float(rg[j]), u = __uint_as_float(ru[j]);
-              float t;
-              asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * g));     // sigmoid(g) = 0.5 + 0.5 tanh(g / 2)
-              hv[j] = g * fmaf(0.5f, t, 0.5f) * u;
-            }
+          for (int g = 0; g < 4; ++g) {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4 o;
-              o.x = pk(hv[8 * j + 0], hv[8 * j + 1]); o.y = pk(hv[8 * j + 2], hv[8 * j + 3]);
-              o.z = pk(hv[8 * j + 4], hv[8 * j + 5]); o.w = pk(hv[8 * j + 6], hv[8 * j + 7]);
-              h4[j] = o;
-            }
-            if (args.gu_out != nullptr) {
-              __nv_bfloat16* gp = reinterpret_cast<__nv_bfloat16*>(args.gu_out) + grow * args.ldgu + gcol;
-              uint4* g4 = reinterpret_cast<uint4*>(gp);
-              uint4* u4 = reinterpret_cast<uint4*>(gp + args.swiglu_F);
+            for (int half = 0; half < 2; ++half) {
+              uint32_t xh[4], xg[4], xu[4];
 #pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                uint4 a, b;
-                a.x = pk(__uint_as_float(rg[8 * j + 0]), __uint_as_float(rg[8 * j + 1]));
-                a.y = pk(__uint_as_float(rg[8 * j + 2]), __uint_as_float(rg[8 * j + 3]));
-                a.z = pk(__uint_as_float(rg[8 * j + 4]), __uint_as_float(rg[8 * j + 5]));
-                a.w = pk(__uint_as_float(rg[8 * j + 6]), __uint_as_float(rg[8 * j + 7]));
-                b.x = pk(__uint_as_float(ru[8 * j + 0]), __uint_as_float(ru[8 * j + 1]));
-                b.y = pk(__uint_as_float(ru[8 * j + 2]), __uint_as_float(ru[8 * j + 3]));
-                b.z = pk(__uint_as_float(ru[8 * j + 4]), __uint_as_float(ru[8 * j + 5]));
-                b.w = pk(__uint_as_float(ru[8 * j + 6]), __uint_as_float(ru[8 * j + 7]));
-                g4[j] = a;
-                u4[j] = b;
+              for (int jj = 0; jj < 4; ++jj) {
+                const int j = 4 * g + jj;
+                float hv[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float gt = acc[4 * j + 2 * half + e], up = acc[4 * (j + 16) + 2 * half + e];
+                  float th;
+                  asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * gt));     // sigmoid(g) = 0.5 + 0.5 tanh(g / 2)
+                  hv[e] = gt * fmaf(0.5f, th, 0.5f) * up;
+                }
+                xh[jj] = pk(hv[0], hv[1]);
+                xg[jj] = pk(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
+                xu[jj] = pk(acc[4 * (j + 16) + 2 * half], acc[4 * (j + 16) + 2 * half + 1]);
+              }
+              quad_transpose(xh, lane);
+              const long long grow = row0 + 8 * half;
+              const int col = tn * (kBlockN / 2) + 32 * g + 8 * (int)quad;   // output column (of F)
+              const bool ok = grow < args.M && col < args.swiglu_F;
+              if (ok) store_row8(reinterpret_cast<uint16_t*>(args.D) + grow * args.ldd + col, xh, args.swiglu_F - col, vec_h);
+              if (args.gu_out != nullptr) {
+                quad_transpose(xg, lane);
+                quad_transpose(xu, lane);
+                if (ok) {
+                  uint16_t* gp = reinterpret_cast<uint16_t*>(args.gu_out) + grow * args.ldgu + col;
+                  store_row8(gp, xg, args.swiglu_F - col, vec_h);
+                  store_row8(gp + args.swiglu_F, xu, args.swiglu_F - col, vec_h);
+                }
               }
             }
           }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cluster(tempty_leader + 8u * as);
           continue;
         }
       }
-#pragma unroll 1
-      for (int c = 0; c < kBlockN / 32; ++c) {
-        __syncwarp();  // tcgen05.ld is warp-collective (.sync.aligned): reconverge after the guarded stores
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + ((q * 32u) << 16) + as * kBlockN + c * 32, r);
-        tmem_ld_wait();
-        const int gcol = n0 + c * 32;
-        if (!row_ok || gcol >= args.N) continue;
-        float v[32];
+      const int n0 = tn * kBlockN;
+      const uint16_t* bias = reinterpret_cast<const uint16_t*>(args.bias);
+      if (args.out_fp32) {
+        // fp32 output: the four lanes of a quad already cover 32 contiguous bytes of a row
+        const bool vec = (args.ldd % 2 == 0) && (args.C == nullptr || args.ldc % 2 == 0) &&
+                         (reinterpret_cast<uintptr_t>(args.D) % 8 == 0) && (reinterpret_cast<uintptr_t>(args.C) % 8 == 0);
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        const bool full = gcol + 32 <= args.N;
-        if (args.bias != nullptr) {
-          if (full) {
-            const uint4* bp = reinterpret_cast<const uint4*>(args.bias + gcol);
+        for (int j = 0; j < kBlockN / 8; ++j) {
+          const int col = n0 + 8 * j + 2 * (int)quad;
+          if (col >= args.N) continue;
+          const bool two = col + 1 < args.N;
+          const float b0 = bias ? ld1(bias + col) : 0.f, b1 = (bias && two) ? ld1(bias + col + 1) : 0.f;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              uint4 b = __ldg(bp + j);
-              float2 f0 = unpk(b.x), f1 = unpk(b.y), f2 = unpk(b.z), f3 = unpk(b.w);
-              v[8 * j + 0] += f0.x; v[8 * j + 1] += f0.y; v[8 * j + 2] += f1.x; v[8 * j + 3] += f1.y;
-              v[8 * j + 4] += f2.x; v[8 * j + 5] += f2.y; v[8 * j + 6] += f3.x; v[8 * j + 7] += f3.y;
+          for (int half = 0; half < 2; ++half) {
+            const long long grow = row0 + 8 * half;
+            if (grow >= args.M) continue;
+            float v0 = acc[4 * j + 2 * half] + b0, v1 = acc[4 * j + 2 * half + 1] + b1;
+            float* dp = reinterpret_cast<float*>(args.D) + grow * args.ldd + col;
+            const float* cp = args.C ? reinterpret_cast<const float*>(args.C) + grow * args.ldc + col : nullptr;
+            if (two && vec) {
+              if (cp) {
+                const float2 old = *reinterpret_cast<const float2*>(cp);
+                v0 += old.x; v1 += old.y;
+              }
+              *reinterpret_cast<float2*>(dp) = make_float2(v0, v1);
+            } else {
+              dp[0] = v0 + (cp ? cp[0] : 0.f);
+              if (two) dp[1] = v1 + (cp ? cp[1] : 0.f);
             }
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (gcol + j < args.N) v[j] += ld1(args.bias + gcol + j);
           }
         }
-        if (args.out_fp32) {
-          float* dp = reinterpret_cast<float*>(args.D) + grow * args.ldd + gcol;
-          const float* cp = args.C ? reinterpret_cast<const float*>(args.C) + grow * args.ldc + gcol : nullptr;
-          if (full) {
-            float4* d4 = reinterpret_cast<float4*>(dp);
-            const float4* c4 = reinterpret_cast<const float4*>(cp);
+      } else {
+        // 16-bit output: bias / addend are applied in fp32 in the accumulator layout, then each quad transposes its
+        // packed pairs so that every lane stores 16 contiguous bytes
+        const bool vec_d = (args.ldd % 8 == 0) && (reinterpret_cast<uintptr_t>(args.D) % 16 == 0);
+        const bool pair_c = args.C != nullptr && (args.ldc % 2 == 0) && (reinterpret_cast<uintptr_t>(args.C) % 4 == 0);
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 o = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              if (cp) {
-                float4 old = c4[j];
-                o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-              }
-              d4[j] = o;
-            }
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (gcol + j < args.N) dp[j] = v[j] + (cp ? cp[j] : 0.f);
-          }
-        } else {
-          __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(args.D) + grow * args.ldd + gcol;
-          const __nv_bfloat16* cp =
-              args.C ? reinterpret_cast<const __nv_bfloat16*>(args.C) + grow * args.ldc + gcol : nullptr;
-          if (full) {
-            uint4* d4 = reinterpret_cast<uint4*>(dp);
-            const uint4* c4 = reinterpret_cast<const uint4*>(cp);
+        for (int g = 0; g < kBlockN / 32; ++g) {
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if (cp) {
-                uint4 old = c4[j];
-                float2 f0 = unpk(old.x), f1 = unpk(old.y), f2 = unpk(old.z), f3 = unpk(old.w);
-                v[8 * j + 0] += f0.x; v[8 * j + 1] += f0.y; v[8 * j + 2] += f1.x; v[8 * j + 3] += f1.y;
-                v[8 * j + 4] += f2.x; v[8 * j + 5] += f2.y; v[8 * j + 6] += f3.x; v[8 * j + 7] += f3.y;
+          for (int half = 0; half < 2; ++half) {
+            const long long grow = row0 + 8 * half;
+            const bool row_ok = grow < args.M;
+            uint32_t x[4];
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * g + jj;
+              const int col = n0 + 8 * j + 2 * (int)quad;
+              float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+              if (row_ok && col < args.N) {
+                const bool two = col + 1 < args.N;
+                if (bias) {
+                  v0 += ld1(bias + col);
+                  if (two) v1 += ld1(bias + col + 1);
+                }
+                if (args.C) {
+                  const uint16_t* cp = reinterpret_cast<const uint16_t*>(args.C) + grow * args.ldc + col;
+                  if (two && pair_c) {
+                    const float2 old = unpack_h2<kBf16>(*reinterpret_cast<const uint32_t*>(cp));
+                    v0 += old.x; v1 += old.y;
+                  } else {
+                    v0 += ld1(cp);
+                    if (two) v1 += ld1(cp + 1);
+                  }
+                }
               }
-              uint4 o;
-              o.x = pk(v[8 * j + 0], v[8 * j + 1]);
-              o.y = pk(v[8 * j + 2], v[8 * j + 3]);
-              o.z = pk(v[8 * j + 4], v[8 * j + 5]);
-              o.w = pk(v[8 * j + 6], v[8 * j + 7]);
-              d4[j] = o;
+              x[jj] = pk(v0, v1);
             }
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (gcol + j < args.N) st1(dp + j, v[j] + (cp ? ld1(cp + j) : 0.f));
+            quad_transpose(x, lane);
+            const int col = n0 + 32 * g + 8 * (int)quad;
+            if (row_ok && col < args.N)
+              store_row8(reinterpret_cast<uint16_t*>(args.D) + grow * args.ldd + col, x, args.N - col, vec_d);
           }
         }
-      }
-      // All TMEM reads of this accumulator stage are complete: hand it back to the MMA warp.
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if constexpr (kCluster == 2) mbar_arrive_cluster(tempty_leader + 8u * as);
-        else mbar_arrive(tempty_leader + 8u * as);
       }
     }
     flush_arrivals();
-  }
-
-  // ================================ Teardown ================================
-  __syncwarp();  // single-lane role loops: reconverge each warp before the aligned barrier
-  tc_fence_before();
-  if constexpr (kCluster == 2) cluster_sync(); else __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<kCluster>(tmem_base, 512);
   }
   if constexpr (kFuse == 0) {
     if (args.carry.debug != nullptr && blockIdx.x == 0 && threadIdx.x == 0) args.carry.debug[7] = carry_now_ns();
@@ -680,11 +547,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // ------------------------------------------------------------------------------------------------------
 // Host launcher
 // ------------------------------------------------------------------------------------------------------
-template <int kCluster, Major kAMajor, Major kBMajor, int kFuse>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, const GemmArgs& args, int num_sms,
                               cudaStream_t stream) {
-  using S = GemmSmem<kCluster>;
-  auto kern = gemm_bf16_kernel<kCluster, kAMajor, kBMajor, kFuse>;
+  using S = GemmSmem;
+  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotalCarry);
@@ -693,31 +560,21 @@ static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, con
   }
   const bool carrying = kFuse == 0 && args.carry.slice[0].kind != 0;
   const int num_tiles = args.num_m_tiles * args.num_n_tiles;
-  int clusters = num_sms / kCluster;
-  if (kFuse == 1) clusters -= args.fuse.comm_clusters;   // copy clusters share their SMs with nobody
-  if (clusters > num_tiles) clusters = num_tiles;
-  if (clusters < 1) clusters = 1;
-  if (kFuse == 1) clusters += args.fuse.comm_clusters;
-  if (kFuse == 0 && args.dynamic) clusters = num_tiles;   // one cluster per tile; extra ones are cancelled on device
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(clusters * kCluster);
-  cfg.blockDim = dim3(kNumThreads);
-  cfg.dynamicSmemBytes = carrying ? S::kTotalCarry : S::kTotal;   // the ring only when there is something to carry
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = kCluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, ta, tb_, args);
+  const int comm_ctas = (kFuse == 1) ? args.fuse.comm_clusters * kCommCtasPerCluster : 0;
+  int ctas = num_sms - comm_ctas;   // copy CTAs share their SMs with nobody
+  if (ctas > num_tiles) ctas = num_tiles;
+  if (ctas < 1) ctas = 1;
+  ctas += comm_ctas;
+  if (kFuse == 0 && args.dynamic) ctas = num_tiles;   // one CTA per tile: the block scheduler hands them to free SMs
+  const int smem = carrying ? S::kTotalCarry : S::kTotal;   // the ring only when there is something to carry
+  kern<<<ctas, kNumThreads, smem, stream>>>(ta, tb_, args);
+  return cudaGetLastError();
 }
 
-// 1 = dynamic (cluster-launch-control) tile scheduling, 0 = static striping.  mode < 0 only queries.
+// 1 = dynamic tile scheduling (one CTA per tile), 0 = static striping over a persistent grid.  mode < 0 only queries.
 int gemm_sched_mode(int mode) {
-  // default static: ~1-3 % faster when the GEMM owns the GPU (profiles/gemm_sched_ab_run21.txt); the sharding engine
-  // switches to dynamic when collectives run next to the GEMMs.  TORCHACC_B200_GEMM_SCHED=static|dynamic pins it.
+  // default static; the sharding engine switches to dynamic when collectives run next to the GEMMs.
+  // TORCHACC_B200_GEMM_SCHED=static|dynamic pins it.
   static int current = [] {
     const char* e = getenv("TORCHACC_B200_GEMM_SCHED");
     return (e && e[0] == 'd') ? 1 : 0;
@@ -727,22 +584,25 @@ int gemm_sched_mode(int mode) {
 }
 
 static bool fill_common(GemmArgs& args, void* D, const void* bias, int M, int N, int K, long long ldd, bool out_fp32,
-                        const void* C, long long ldc, int cluster) {
+                        const void* C, long long ldc) {
   args.D = D;
   args.bias = reinterpret_cast<const __nv_bfloat16*>(bias);
   args.M = M; args.N = N; args.K = K;
   args.ldd = ldd;
   args.C = C; args.ldc = ldc;
   args.out_fp32 = out_fp32 ? 1 : 0;
-  const int tile_m = kBlockMCta * cluster;
-  args.num_m_tiles = (M + tile_m - 1) / tile_m;
+  args.num_m_tiles = (M + kBlockM - 1) / kBlockM;
   args.num_n_tiles = (N + kBlockN - 1) / kBlockN;
   args.dynamic = gemm_sched_mode(-1);
-  args.fp16 = 0;
   args.swiglu = 0; args.swiglu_F = 0; args.gu_out = nullptr; args.ldgu = 0;
   memset(&args.fuse, 0, sizeof(args.fuse));
   memset(&args.carry, 0, sizeof(args.carry));
   return true;
+}
+
+// K-major: matrix [MN][K], box 64 x box_rows; MN-major: matrix [K][MN], box 64 (MN) x 64 (K).  Inner box = 128 B.
+static CUtensorMap operand_map(const void* p, int mn, int K, long long ld, bool mn_major, int box_rows) {
+  return mn_major ? make_map_2d_bf16(p, K, mn, ld, 64, kBlockK) : make_map_2d_bf16(p, mn, K, ld, kBlockK, box_rows);
 }
 
 cudaError_t gemm_bf16(const void* A, const void* B, void* D, const void* bias, int M, int N, int K, long long lda,
@@ -758,35 +618,31 @@ cudaError_t gemm_bf16_ex(const void* A, const void* B, void* D, const void* bias
   if (M <= 0 || N <= 0) return cudaSuccess;
   if (K <= 0) return cudaErrorInvalidValue;
   if (cluster != 1 && cluster != 2) return cudaErrorInvalidValue;
-  const int load_n = kBlockN / cluster;
   CUtensorMap ta, tbm;
   try {
-    // K-major: matrix [MN][K]; MN-major: matrix [K][MN].  Inner box is always 64 elements = 128 B.
-    ta = a_mn_major ? make_map_2d_bf16(A, K, M, lda, 64, kBlockK) : make_map_2d_bf16(A, M, K, lda, kBlockK, kBlockMCta);
-    tbm = b_mn_major ? make_map_2d_bf16(B, K, N, ldb, 64, kBlockK) : make_map_2d_bf16(B, N, K, ldb, kBlockK, load_n);
+    ta = operand_map(A, M, K, lda, a_mn_major, kBlockM);
+    tbm = operand_map(B, N, K, ldb, b_mn_major, kBlockN / 2);
   } catch (const std::exception& e) {
     fprintf(stderr, "%s\n", e.what());
     return cudaErrorInvalidValue;
   }
   GemmArgs args;
-  fill_common(args, D, bias, M, N, K, ldd, out_fp32, C, ldc, cluster);
-  args.fp16 = is_fp16 ? 1 : 0;
+  fill_common(args, D, bias, M, N, K, ldd, out_fp32, C, ldc);
   // pending FSDP collectives ride along: bytes proportional to this GEMM's FLOPs (static scheduling only -- under
-  // dynamic scheduling warp 3 is the tile scheduler and collectives run as their own kernels)
+  // dynamic scheduling the collectives run as their own kernels)
   if (!args.dynamic) carry_take(2.0 * (double)M * (double)N * (double)K, &args.carry);
 
-#define TB_DISPATCH(CL, AM, BM) return launch_one<CL, AM, BM, 0>(ta, tbm, args, num_sms, stream)
-  if (cluster == 2) {
-    if (!a_mn_major && !b_mn_major) TB_DISPATCH(2, Major::K, Major::K);
-    if (!a_mn_major && b_mn_major) TB_DISPATCH(2, Major::K, Major::MN);
-    if (a_mn_major && !b_mn_major) TB_DISPATCH(2, Major::MN, Major::K);
-    TB_DISPATCH(2, Major::MN, Major::MN);
-  } else {
-    if (!a_mn_major && !b_mn_major) TB_DISPATCH(1, Major::K, Major::K);
-    if (!a_mn_major && b_mn_major) TB_DISPATCH(1, Major::K, Major::MN);
-    if (a_mn_major && !b_mn_major) TB_DISPATCH(1, Major::MN, Major::K);
-    TB_DISPATCH(1, Major::MN, Major::MN);
+#define TB_DISPATCH(BF, AM, BM) return launch_one<BF, AM, BM, 0>(ta, tbm, args, num_sms, stream)
+#define TB_MAJORS(BF)                                                  \
+  if (!a_mn_major && !b_mn_major) TB_DISPATCH(BF, Major::K, Major::K); \
+  if (!a_mn_major && b_mn_major) TB_DISPATCH(BF, Major::K, Major::MN); \
+  if (a_mn_major && !b_mn_major) TB_DISPATCH(BF, Major::MN, Major::K); \
+  TB_DISPATCH(BF, Major::MN, Major::MN)
+  if (is_fp16) {
+    TB_MAJORS(false);
   }
+  TB_MAJORS(true);
+#undef TB_MAJORS
 #undef TB_DISPATCH
 }
 
@@ -796,30 +652,31 @@ cudaError_t gemm_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, 
                              bool is_fp16) {
   if (M <= 0 || F <= 0) return cudaSuccess;
   if (K <= 0 || F % 128 != 0 || ldh % 8 != 0 || (GU != nullptr && ldgu % 8 != 0)) return cudaErrorInvalidValue;
+  if (reinterpret_cast<uintptr_t>(H) % 16 != 0 || reinterpret_cast<uintptr_t>(GU) % 16 != 0) return cudaErrorInvalidValue;
   CUtensorMap ta, tbm;
   try {
-    ta = make_map_2d_bf16(A, M, K, lda, kBlockK, kBlockMCta);
+    ta = make_map_2d_bf16(A, M, K, lda, kBlockK, kBlockM);
     tbm = make_map_2d_bf16(Wgu, 2 * (uint64_t)F, K, ldb, kBlockK, kBlockN / 2);
   } catch (const std::exception& e) {
     fprintf(stderr, "%s\n", e.what());
     return cudaErrorInvalidValue;
   }
   GemmArgs args;
-  fill_common(args, H, nullptr, M, F, K, ldh, false, nullptr, 0, 2);
+  fill_common(args, H, nullptr, M, F, K, ldh, false, nullptr, 0);
   args.num_n_tiles = F / 128;           // each 256-wide accumulator tile yields 128 output columns
   args.swiglu = 1; args.swiglu_F = F; args.gu_out = GU; args.ldgu = ldgu;
-  args.fp16 = is_fp16 ? 1 : 0;
-  args.dynamic = 0;                      // the gate/up row pairing relies on the static pair layout
+  args.dynamic = 0;
   carry_take(4.0 * (double)M * (double)F * (double)K, &args.carry);
-  return launch_one<2, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
+  if (is_fp16) return launch_one<false, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
+  return launch_one<true, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------
-// Fused tensor-parallel entry points (cta_group::2 kernels only)
+// Fused tensor-parallel entry points
 // ------------------------------------------------------------------------------------------------------
 static cudaError_t check_fused(int world, int rows_per_rank, int N, int channel) {
   if (world < 2 || world > kMaxPeers || channel < 0 || channel >= 64) return cudaErrorInvalidValue;
-  if (rows_per_rank % (kBlockMCta * 2) != 0) return cudaErrorInvalidValue;   // M tiles must not straddle ranks
+  if (rows_per_rank % (kBlockM * 2) != 0) return cudaErrorInvalidValue;   // M tiles must not straddle ranks
   if (N % 8 != 0) return cudaErrorInvalidValue;
   return cudaSuccess;
 }
@@ -831,18 +688,18 @@ cudaError_t ag_gemm_bf16(const uint64_t* peer_a_full, const uint64_t* pad_ptrs, 
                          cudaStream_t stream) {
   cudaError_t e = check_fused(world, rows_per_rank, N, channel);
   if (e != cudaSuccess) return e;
-  if (K % 8 != 0 || comm_clusters < 1 || comm_clusters * 2 >= num_sms) return cudaErrorInvalidValue;
+  if (K % 8 != 0 || comm_clusters < 1 || comm_clusters * kCommCtasPerCluster >= num_sms) return cudaErrorInvalidValue;
   const int M = rows_per_rank * world;
   CUtensorMap ta, tbm;
   try {
-    ta = make_map_2d_bf16(a_full, M, K, K, kBlockK, kBlockMCta);
-    tbm = b_mn_major ? make_map_2d_bf16(B, K, N, ldb, 64, kBlockK) : make_map_2d_bf16(B, N, K, ldb, kBlockK, kBlockN / 2);
+    ta = make_map_2d_bf16(a_full, M, K, K, kBlockK, kBlockM);
+    tbm = operand_map(B, N, K, ldb, b_mn_major, kBlockN / 2);
   } catch (const std::exception& ex) {
     fprintf(stderr, "%s\n", ex.what());
     return cudaErrorInvalidValue;
   }
   GemmArgs args;
-  fill_common(args, D, bias, M, N, K, ldd, false, nullptr, 0, 2);
+  fill_common(args, D, bias, M, N, K, ldd, false, nullptr, 0);
   FuseArgs& f = args.fuse;
   for (int i = 0; i < world; ++i) {
     f.peer[i] = reinterpret_cast<void*>(peer_a_full[i]);
@@ -851,8 +708,8 @@ cudaError_t ag_gemm_bf16(const uint64_t* peer_a_full, const uint64_t* pad_ptrs, 
   f.a_full = a_full; f.flags = flags; f.block_counter = block_counter;
   f.rank = rank; f.world = world; f.rows_per_rank = rows_per_rank; f.channel = channel;
   f.epoch = epoch; f.flag_target = flag_target; f.comm_clusters = comm_clusters;
-  if (b_mn_major) return launch_one<2, Major::K, Major::MN, 1>(ta, tbm, args, num_sms, stream);
-  return launch_one<2, Major::K, Major::K, 1>(ta, tbm, args, num_sms, stream);
+  if (b_mn_major) return launch_one<true, Major::K, Major::MN, 1>(ta, tbm, args, num_sms, stream);
+  return launch_one<true, Major::K, Major::K, 1>(ta, tbm, args, num_sms, stream);
 }
 
 cudaError_t gemm_rs_bf16(const void* A, const void* B, const uint64_t* peer_stage, const uint64_t* peer_counters,
@@ -865,14 +722,14 @@ cudaError_t gemm_rs_bf16(const void* A, const void* B, const uint64_t* peer_stag
   const int M = rows_per_rank * world;
   CUtensorMap ta, tbm;
   try {
-    ta = a_mn_major ? make_map_2d_bf16(A, K, M, lda, 64, kBlockK) : make_map_2d_bf16(A, M, K, lda, kBlockK, kBlockMCta);
-    tbm = b_mn_major ? make_map_2d_bf16(B, K, N, ldb, 64, kBlockK) : make_map_2d_bf16(B, N, K, ldb, kBlockK, kBlockN / 2);
+    ta = operand_map(A, M, K, lda, a_mn_major, kBlockM);
+    tbm = operand_map(B, N, K, ldb, b_mn_major, kBlockN / 2);
   } catch (const std::exception& ex) {
     fprintf(stderr, "%s\n", ex.what());
     return cudaErrorInvalidValue;
   }
   GemmArgs args;
-  fill_common(args, nullptr, nullptr, M, N, K, /*ldd=*/N, false, nullptr, 0, 2);
+  fill_common(args, nullptr, nullptr, M, N, K, /*ldd=*/N, false, nullptr, 0);
   FuseArgs& f = args.fuse;
   for (int i = 0; i < world; ++i) {
     f.peer[i] = reinterpret_cast<void*>(peer_stage[i]);
@@ -880,8 +737,8 @@ cudaError_t gemm_rs_bf16(const void* A, const void* B, const uint64_t* peer_stag
     f.pads[i] = reinterpret_cast<uint32_t*>(pad_ptrs[i]);
   }
   f.rank = rank; f.world = world; f.rows_per_rank = rows_per_rank; f.channel = channel; f.epoch = epoch;
-  f.slot_stride = (long long)rows_per_rank * ((N + kBlockN - 1) / kBlockN * kBlockN);   // block-major, padded N
-#define TB_RS(AM, BM) return launch_one<2, AM, BM, 2>(ta, tbm, args, num_sms, stream)
+  f.slot_stride = (long long)rows_per_rank * ((N + kBlockN - 1) / kBlockN * kBlockN);   // row-major, padded N
+#define TB_RS(AM, BM) return launch_one<true, AM, BM, 2>(ta, tbm, args, num_sms, stream)
   if (!a_mn_major && !b_mn_major) TB_RS(Major::K, Major::K);
   if (!a_mn_major && b_mn_major) TB_RS(Major::K, Major::MN);
   if (a_mn_major && !b_mn_major) TB_RS(Major::MN, Major::K);
@@ -890,8 +747,7 @@ cudaError_t gemm_rs_bf16(const void* A, const void* B, const uint64_t* peer_stag
 }
 
 // out[rows, N] = sum_src stage[src] (+ residual), once every source has delivered `expected` arrivals.
-// Staging slots are block-major (see the kFuse == 2 epilogue): one warp handles one 2 KB block = 32 rows x 32 columns;
-// its four loads per source are 512-byte coalesced, each lane then owns 64 contiguous output bytes of one row.
+// Staging slots are row-major with the row pitch padded to the GEMM's 256-column tile; one thread sums 8 columns.
 __global__ void __launch_bounds__(256)
 rs_reduce_kernel(const __nv_bfloat16* __restrict__ stage, const uint32_t* __restrict__ counters, uint32_t expected,
                  const __nv_bfloat16* __restrict__ residual, __nv_bfloat16* __restrict__ out, int rows, int N, int world,
@@ -899,52 +755,26 @@ rs_reduce_kernel(const __nv_bfloat16* __restrict__ stage, const uint32_t* __rest
   if (threadIdx.x < world)
     spin_until_count(counters + threadIdx.x, expected, -1, (int)threadIdx.x, "GEMM -> reduce-scatter arrivals");
   __syncthreads();
-  const int num_n_tiles = (N + 255) / 256;
-  const long long num_blocks = (long long)(rows / 256) * num_n_tiles * 64;
-  const int lane = threadIdx.x & 31;
-  const long long warps = (long long)gridDim.x * (blockDim.x >> 5);
-  for (long long w = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5); w < num_blocks; w += warps) {
-    const int c = (int)(w & 7), q = (int)((w >> 3) & 3), cta = (int)((w >> 5) & 1);
-    const long long tile = w >> 6;
-    const int tn = (int)(tile % num_n_tiles);
-    const long long tm = tile / num_n_tiles;
-    const int col = tn * 256 + c * 32;
-    if (col + 32 > N) continue;
-    const long long row = tm * 256 + cta * 128 + q * 32 + lane;
-    float acc[32];
+  const long long npad = (long long)((N + kBlockN - 1) / kBlockN) * kBlockN;
+  const int vecs = N / 8;
+  const long long total = (long long)rows * vecs;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long row = i / vecs;
+    const int col = (int)(i % vecs) * 8;
+    float acc[8];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-    for (int s = 0; s < world; ++s) {
-      const uint4* src = reinterpret_cast<const uint4*>(stage + s * slot_stride) + w * 128 + lane;
-      uint4 u[4];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) u[j] = ld_volatile_v4(src + j * 32);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float2 a = unpack_bf16x2(u[j].x), b = unpack_bf16x2(u[j].y), cc = unpack_bf16x2(u[j].z), d = unpack_bf16x2(u[j].w);
-        acc[8 * j + 0] += a.x; acc[8 * j + 1] += a.y; acc[8 * j + 2] += b.x; acc[8 * j + 3] += b.y;
-        acc[8 * j + 4] += cc.x; acc[8 * j + 5] += cc.y; acc[8 * j + 6] += d.x; acc[8 * j + 7] += d.y;
-      }
-    }
-    const long long o_off = row * N + col;
-    if (residual) {
-      const uint4* rp = reinterpret_cast<const uint4*>(residual + o_off);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint4 u = rp[j];
-        float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), cc = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-        acc[8 * j + 0] += a.x; acc[8 * j + 1] += a.y; acc[8 * j + 2] += b.x; acc[8 * j + 3] += b.y;
-        acc[8 * j + 4] += cc.x; acc[8 * j + 5] += cc.y; acc[8 * j + 6] += d.x; acc[8 * j + 7] += d.y;
-      }
-    }
-    uint4* op = reinterpret_cast<uint4*>(out + o_off);
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint4 o;
-      o.x = pack_bf16x2(acc[8 * j + 0], acc[8 * j + 1]); o.y = pack_bf16x2(acc[8 * j + 2], acc[8 * j + 3]);
-      o.z = pack_bf16x2(acc[8 * j + 4], acc[8 * j + 5]); o.w = pack_bf16x2(acc[8 * j + 6], acc[8 * j + 7]);
-      op[j] = o;
-    }
+    for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+    auto add = [&](const uint4& u) {
+      float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
+      acc[0] += a.x; acc[1] += a.y; acc[2] += b.x; acc[3] += b.y;
+      acc[4] += c.x; acc[5] += c.y; acc[6] += d.x; acc[7] += d.y;
+    };
+    for (int s = 0; s < world; ++s) add(ld_volatile_v4(stage + s * slot_stride + row * npad + col));
+    if (residual) add(*reinterpret_cast<const uint4*>(residual + row * N + col));
+    uint4 o;
+    o.x = pack_bf16x2(acc[0], acc[1]); o.y = pack_bf16x2(acc[2], acc[3]);
+    o.z = pack_bf16x2(acc[4], acc[5]); o.w = pack_bf16x2(acc[6], acc[7]);
+    *reinterpret_cast<uint4*>(out + row * N + col) = o;
   }
 }
 
@@ -952,7 +782,7 @@ cudaError_t rs_reduce_bf16(const void* stage, const uint32_t* counters, uint32_t
                            void* out, int rows, int N, int world, long long slot_stride, int num_sms,
                            cudaStream_t stream) {
   if (N % 32 != 0 || rows % 256 != 0) return cudaErrorInvalidValue;
-  long long blocks = (long long)(rows / 256) * ((N + 255) / 256) * 64 / 8;   // 8 warps per CTA
+  long long blocks = ((long long)rows * (N / 8) + 255) / 256;
   if (blocks > (long long)num_sms * 4) blocks = (long long)num_sms * 4;
   if (blocks < 1) blocks = 1;
   rs_reduce_kernel<<<(unsigned)blocks, 256, 0, stream>>>((const __nv_bfloat16*)stage, counters, expected,

@@ -1,18 +1,15 @@
-// Block-scaled FP8 (MX: e4m3 elements, one UE8M0 scale per 32 elements along K) GEMM on tcgen05 for sm_100a.
+// Block-scaled FP8 (MX: e4m3 elements, one UE8M0 scale per 32 elements along K) GEMM on wgmma for sm_90a.
 //
 //   D[M,N] (bf16 or fp32, row-major) (+)= (A[M,K] * SFA) . (B[N,K] * SFB)^T        A, B: e4m3, K-major
 //
-// tcgen05.mma.kind::mxf8f6f4.block_scale applies the scales inside the tensor core: for every K block of 32 elements
-// the hardware multiplies the partial dot product by 2^(sfa-127) * 2^(sfb-127), with the scale bytes read from tensor
-// memory.  Per pipeline stage (K = 128 elements = one 128-byte swizzle row, i.e. the SAME smem tile bytes and UMMA
-// descriptors as the bf16 kernel at twice the FLOPs):
-//   warp 0 : TMA producer  -- A tile 128 x 128 B, B tile 192 x 128 B (SWIZZLE_128B), plus the scale "atoms" of the stage
-//            (512 B for 128 rows x 4 K-blocks, layout of cutlass::detail::Sm1xxBlockScaledBasicChunk) as bulk copies
-//   warp 1 : MMA issuer    -- tcgen05.cp the scale atoms smem -> TMEM (32x128b.warpx4: each 16-byte line holds the 4
-//            K-block scales of rows r, r+32, r+64, r+96 and lands in the 4 lane quarters), then 4 x
-//            tcgen05.mma 128x192x32 with a_sf_id = b_sf_id = K-block index inside the atom
-//   warp 2 : TMEM allocator (512 columns: 2 x 192 accumulator + 2 x (4 SFA + 8 SFB) scale columns)
-//   warps 4-7 : epilogue   -- tcgen05.ld -> (+ C) -> bf16/fp32 stores; double-buffered against the next tile's mainloop
+// Hopper's tensor cores multiply e4m3 operands but know nothing about block scales, and one wgmma.m64n128k32 covers
+// exactly one 32-element scale block.  So every K block of 32 is multiplied into a scratch accumulator and promoted into
+// the fp32 result with the factor 2^(sfa-127) * 2^(sfb-127) of its (row, column) -- a power of two, so the promotion is
+// exact.  Per pipeline stage (K = 128 elements = one 128-byte swizzle row):
+//   warp 0     : TMA producer -- A tile 128 x 128 B, B tile 128 x 128 B (SWIZZLE_128B), plus the two scale "atoms" of the
+//                stage (512 B for 128 rows x 4 K-blocks, layout written by ops/quant_mxfp8.cu) as bulk copies
+//   warps 4-11 : two MMA warpgroups (64 rows each): 4 x (wgmma 64x128x32 -> scale -> accumulate), then the epilogue
+//                (+ C) -> bf16/fp32 stores
 // All three GEMMs of a linear layer are K-major x K-major here: the transposed operands of dgrad / wgrad come from the
 // transposing quantiser (ops/quant_mxfp8.cu), because the scales must run along the contraction dimension.
 //
@@ -28,21 +25,17 @@ namespace tb {
 
 namespace mx {
 
-constexpr int kBM = 128, kBN = 192, kBKBytes = 128;   // tile; K block = 128 e4m3 elements
+constexpr int kBM = 128, kBN = 128, kBKBytes = 128;   // tile; K block = 128 e4m3 elements
 constexpr int kStages = 5;
-constexpr int kThreads = 256;
+constexpr int kThreads = 384;
 constexpr int kABytes = kBM * kBKBytes;               // 16 KB
-constexpr int kBBytes = kBN * kBKBytes;               // 24 KB
-constexpr int kSfaBytes = 512, kSfbBytes = 1024;      // 1 atom (128 rows) / 2 atoms (covers any 192-row window)
+constexpr int kBBytes = kBN * kBKBytes;               // 16 KB
+constexpr int kSfBytes = 512;                         // one atom: 128 rows x 4 K blocks
 constexpr int kStageBytes = kABytes + kBBytes;
-constexpr int kSfStageBytes = kSfaBytes + kSfbBytes;
+constexpr int kSfStageBytes = 2 * kSfBytes;
 constexpr int kBarBytes = 1024;
 constexpr int kSmemTotal = kStages * kStageBytes + kStages * kSfStageBytes + kBarBytes + 1024;
 constexpr int kGroupM = 8;
-// TMEM columns
-constexpr uint32_t kAccCols = kBN;                    // per accumulator stage
-constexpr uint32_t kSfBase = 2 * kAccCols;            // 384
-constexpr uint32_t kSfSlotCols = 16;                  // 4 (SFA) + 8 (SFB), padded
 
 struct Args {
   void* D;
@@ -52,38 +45,8 @@ struct Args {
   int out_fp32;
   int num_m_tiles, num_n_tiles;
   const uint8_t* sfa;   // atom-tiled: [ceil(M/128)][K/128][512]
-  const uint8_t* sfb;   // atom-tiled: [ceil(N/128) + 1][K/128][512]
+  const uint8_t* sfb;   // atom-tiled: [ceil(N/128)][K/128][512]
 };
-
-// Instruction descriptor of kind::mxf8f6f4.block_scale (cute/arch/mma_sm100_desc.hpp, InstrDescriptorBlockScaled):
-//   [4,6) b_sf_id | [7,10) a_format (0 = e4m3) | [10,13) b_format | 15 a_major | 16 b_major (0 = K) | [17,23) N>>3 |
-//   23 scale_format (1 = ue8m0) | [24,29) M>>4 | [29,31) a_sf_id | 31 k_size (0 = K32)
-__host__ __device__ constexpr uint32_t idesc_mxf8(uint32_t m, uint32_t n) {
-  return ((n >> 3) << 17) | (1u << 23) | ((m >> 4) << 24);
-}
-
-TB_DEVICE void umma_mxf8(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t tsfa,
-                         uint32_t tsfb, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%5], [%6], p;\n\t"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate), "r"(tsfa), "r"(tsfb)
-      : "memory");
-}
-
-// smem -> TMEM copy of one scale atom: 32 lines of 16 bytes, replicated into the four 32-lane quarters.
-// Source descriptor: no swizzle, 8-line core matrices of 128 bytes stacked every 128 bytes.
-TB_DEVICE void utccp_sf_atom(uint32_t tmem_col_addr, uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
-  d |= static_cast<uint64_t>((16u >> 4) & 0x3FFFu) << 16;     // leading byte offset (one 16-byte column only)
-  d |= static_cast<uint64_t>((128u >> 4) & 0x3FFFu) << 32;    // stride byte offset: next 8 lines
-  d |= 1ull << 46;                                            // descriptor version (Blackwell)
-  asm volatile("tcgen05.cp.cta_group::1.32x128b.warpx4 [%0], %1;" ::"r"(tmem_col_addr), "l"(d) : "memory");
-}
 
 __device__ __forceinline__ void tile_coords(int t, int num_m_tiles, int num_n_tiles, int& tm, int& tn) {
   const int per_group = kGroupM * num_n_tiles;
@@ -95,6 +58,17 @@ __device__ __forceinline__ void tile_coords(int t, int num_m_tiles, int num_n_ti
   tn = r / gsize;
 }
 
+// the four UE8M0 scales (K blocks 0-3 of the stage) of row r of a 128-row atom
+TB_DEVICE uint32_t ld_sf4(uint32_t atom, int r) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(atom + (uint32_t)((r & 31) * 16 + (r >> 5) * 4)));
+  return v;
+}
+TB_DEVICE float sf_value(uint32_t sf4, int kq) {   // 2^(e-127); e == 0 is the subnormal 2^-127
+  const uint32_t e = (sf4 >> (8 * kq)) & 0xffu;
+  return __uint_as_float(e != 0 ? e << 23 : 0x00400000u);
+}
+
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const Args args) {
@@ -104,13 +78,10 @@ gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const uint32_t bar_base = sf_base + kStages * kSfStageBytes;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (kStages + s); };
-  auto tfull_bar = [&](int s) { return bar_base + 8u * (2 * kStages + s); };
-  auto tempty_bar = [&](int s) { return bar_base + 8u * (2 * kStages + 2 + s); };
-  const uint32_t tmem_slot = bar_base + 8u * (2 * kStages + 4);
   auto smem_a = [&](int s) { return smem_base + s * kStageBytes; };
   auto smem_b = [&](int s) { return smem_base + s * kStageBytes + kABytes; };
   auto smem_sfa = [&](int s) { return sf_base + s * kSfStageBytes; };
-  auto smem_sfb = [&](int s) { return sf_base + s * kSfStageBytes + kSfaBytes; };
+  auto smem_sfb = [&](int s) { return sf_base + s * kSfStageBytes + kSfBytes; };
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const uint32_t lane = lane_id();
@@ -124,160 +95,133 @@ gemm_mxfp8_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (warp_idx == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tfull_bar(s), 1);
-      mbar_init(tempty_bar(s), 4);
+      mbar_init(empty_bar(s), 2);   // one arrival per MMA warpgroup
     }
     fence_mbar_init();
   }
-  if (warp_idx == 2) tmem_alloc<1>(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
 
-  if (warp_idx == 0) {
+  if (warp_idx < 4) {
+    setmaxnreg_dec<40>();
     // ================================ TMA producer ================================
-    if (lane == 0) {
+    if (warp_idx == 0 && lane == 0) {
       int it = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
         int tm, tn;
         tile_coords(t, args.num_m_tiles, args.num_n_tiles, tm, tn);
-        const int m0 = tm * kBM, n0 = tn * kBN;
-        const int atom_b = n0 / 128;                       // first scale atom of B touched by this tile
         for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
           const int s = it % kStages;
           mbar_wait(empty_bar(s), ((it / kStages) & 1) ^ 1);
           mbar_arrive_expect_tx(full_bar(s), kStageBytes + kSfStageBytes);
-          tma_load_2d(smem_a(s), &tmap_a, full_bar(s), kb * kBKBytes, m0);
-          tma_load_2d(smem_b(s), &tmap_b, full_bar(s), kb * kBKBytes, n0);
-          bulk_load(smem_sfa(s), args.sfa + ((size_t)tm * num_k_blocks + kb) * 512, kSfaBytes, full_bar(s));
-          bulk_load(smem_sfb(s), args.sfb + ((size_t)atom_b * num_k_blocks + kb) * 512, 512, full_bar(s));
-          bulk_load(smem_sfb(s) + 512, args.sfb + ((size_t)(atom_b + 1) * num_k_blocks + kb) * 512, 512, full_bar(s));
+          tma_load_2d(smem_a(s), &tmap_a, full_bar(s), kb * kBKBytes, tm * kBM);
+          tma_load_2d(smem_b(s), &tmap_b, full_bar(s), kb * kBKBytes, tn * kBN);
+          bulk_load(smem_sfa(s), args.sfa + ((size_t)tm * num_k_blocks + kb) * 512, kSfBytes, full_bar(s));
+          bulk_load(smem_sfb(s), args.sfb + ((size_t)tn * num_k_blocks + kb) * 512, kSfBytes, full_bar(s));
         }
       }
     }
-  } else if (warp_idx == 1) {
-    // ================================ MMA issuer ================================
-    if (lane == 0) {
-      constexpr uint32_t kIdesc = idesc_mxf8(kBM, kBN);
-      int it = 0, lt = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++lt) {
-        int tm, tn;
-        tile_coords(t, args.num_m_tiles, args.num_n_tiles, tm, tn);
-        const uint32_t sfb_col_off = (uint32_t)((tn * kBN) % 128) / 32;     // tile starts at row 0 or 64 of its atom
-        const int as = lt & 1;
-        mbar_wait(tempty_bar(as), ((lt >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * kAccCols;
-        for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
-          const int s = it % kStages;
-          mbar_wait(full_bar(s), (it / kStages) & 1);
-          tc_fence_after();
-          const uint32_t slot = tmem_base + kSfBase + (uint32_t)(it & 1) * kSfSlotCols;
-          utccp_sf_atom(slot, smem_sfa(s));
-          utccp_sf_atom(slot + 4, smem_sfb(s));
-          utccp_sf_atom(slot + 8, smem_sfb(s) + 512);
-#pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) {
-            const uint64_t da = desc_kmajor_sw128(smem_a(s), k);
-            const uint64_t db = desc_kmajor_sw128(smem_b(s), k);
-            const uint32_t idesc = kIdesc | (k << 4) | (k << 29);           // b_sf_id, a_sf_id = K block in the atom
-            umma_mxf8(tmem_d, da, db, idesc, slot, slot + 4 + sfb_col_off, (uint32_t)((kb | (int)k) != 0));
-          }
-          umma_commit(empty_bar(s));
-        }
-        umma_commit(tfull_bar(as));
-      }
-    }
-  } else if (warp_idx >= 4) {
-    // ================================ Epilogue ================================
-    const uint32_t q = warp_idx & 3;
-    int lt = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++lt) {
-      int tm, tn;
-      tile_coords(t, args.num_m_tiles, args.num_n_tiles, tm, tn);
-      const int as = lt & 1;
-      mbar_wait(tfull_bar(as), (lt >> 1) & 1);
-      tc_fence_after();
-      const long long grow = (long long)tm * kBM + q * 32 + lane;
-      const int n0 = tn * kBN;
-      const bool row_ok = grow < args.M;
-#pragma unroll 1
-      for (int c = 0; c < kBN / 32; ++c) {
-        __syncwarp();
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(tmem_base + ((q * 32u) << 16) + as * kAccCols + c * 32, r);
-        tmem_ld_wait();
-        const int gcol = n0 + c * 32;
-        if (!row_ok || gcol >= args.N) continue;
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        const bool full = gcol + 32 <= args.N;
-        if (args.out_fp32) {
-          float* dp = reinterpret_cast<float*>(args.D) + grow * args.ldd + gcol;
-          const float* cp = args.C ? reinterpret_cast<const float*>(args.C) + grow * args.ldc + gcol : nullptr;
-          if (full) {
-            float4* d4 = reinterpret_cast<float4*>(dp);
-            const float4* c4 = reinterpret_cast<const float4*>(cp);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 o = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-              if (cp) {
-                const float4 old = c4[j];
-                o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-              }
-              d4[j] = o;
-            }
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (gcol + j < args.N) dp[j] = v[j] + (cp ? cp[j] : 0.f);
-          }
-        } else {
-          __nv_bfloat16* dp = reinterpret_cast<__nv_bfloat16*>(args.D) + grow * args.ldd + gcol;
-          const __nv_bfloat16* cp =
-              args.C ? reinterpret_cast<const __nv_bfloat16*>(args.C) + grow * args.ldc + gcol : nullptr;
-          if (full) {
-            uint4* d4 = reinterpret_cast<uint4*>(dp);
-            const uint4* c4 = reinterpret_cast<const uint4*>(cp);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              if (cp) {
-                const uint4 old = c4[j];
-                float2 f0 = unpack_bf16x2(old.x), f1 = unpack_bf16x2(old.y), f2 = unpack_bf16x2(old.z),
-                       f3 = unpack_bf16x2(old.w);
-                v[8 * j + 0] += f0.x; v[8 * j + 1] += f0.y; v[8 * j + 2] += f1.x; v[8 * j + 3] += f1.y;
-                v[8 * j + 4] += f2.x; v[8 * j + 5] += f2.y; v[8 * j + 6] += f3.x; v[8 * j + 7] += f3.y;
-              }
-              uint4 o;
-              o.x = pack_bf16x2(v[8 * j + 0], v[8 * j + 1]);
-              o.y = pack_bf16x2(v[8 * j + 2], v[8 * j + 3]);
-              o.z = pack_bf16x2(v[8 * j + 4], v[8 * j + 5]);
-              o.w = pack_bf16x2(v[8 * j + 6], v[8 * j + 7]);
-              d4[j] = o;
-            }
-          } else {
-            for (int j = 0; j < 32; ++j)
-              if (gcol + j < args.N) dp[j] = __float2bfloat16(v[j] + (cp ? __bfloat162float(cp[j]) : 0.f));
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(as));
-    }
+    return;
   }
 
-  __syncwarp();
-  tc_fence_before();
-  __syncthreads();
-  if (warp_idx == 2) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
+  // ================================ MMA + promotion + epilogue ================================
+  setmaxnreg_inc<232>();
+  const int wg = (warp_idx >> 2) - 1;
+  const uint32_t quad = lane & 3;
+  const int frag_row = wg * 64 + (warp_idx & 3) * 16 + (int)(lane >> 2);   // rows frag_row, frag_row + 8 of the tile
+  int it = 0;
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    int tm, tn;
+    tile_coords(t, args.num_m_tiles, args.num_n_tiles, tm, tn);
+    float acc[kBN / 2];
+#pragma unroll
+    for (int i = 0; i < kBN / 2; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
+      const int s = it % kStages;
+      mbar_wait(full_bar(s), (it / kStages) & 1);
+      const uint32_t sa4[2] = {ld_sf4(smem_sfa(s), frag_row), ld_sf4(smem_sfa(s), frag_row + 8)};
+#pragma unroll
+      for (int kq = 0; kq < 4; ++kq) {
+        float part[kBN / 2];
+        wgmma_fence_acc(part);
+        wgmma_fence();
+        wgmma_ss_e4m3_n128(part, desc_kmajor_sw128(smem_a(s) + wg * 8192, kq), desc_kmajor_sw128(smem_b(s), kq), 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_acc(part);
+        const float sa0 = sf_value(sa4[0], kq), sa1 = sf_value(sa4[1], kq);
+#pragma unroll
+        for (int j = 0; j < kBN / 8; ++j) {
+          const int c = 8 * j + 2 * (int)quad;
+          const float sb0 = sf_value(ld_sf4(smem_sfb(s), c), kq), sb1 = sf_value(ld_sf4(smem_sfb(s), c + 1), kq);
+          acc[4 * j + 0] = fmaf(part[4 * j + 0], sa0 * sb0, acc[4 * j + 0]);
+          acc[4 * j + 1] = fmaf(part[4 * j + 1], sa0 * sb1, acc[4 * j + 1]);
+          acc[4 * j + 2] = fmaf(part[4 * j + 2], sa1 * sb0, acc[4 * j + 2]);
+          acc[4 * j + 3] = fmaf(part[4 * j + 3], sa1 * sb1, acc[4 * j + 3]);
+        }
+      }
+      __syncwarp();
+      // every thread of the group has finished reading the stage (its MMAs retired and its scales are in registers)
+      if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar(s));
+    }
+
+    const long long row0 = (long long)tm * kBM + frag_row;
+    const int n0 = tn * kBN;
+    if (args.out_fp32) {
+      const bool vec = (args.ldd % 2 == 0) && (args.C == nullptr || args.ldc % 2 == 0) &&
+                       (reinterpret_cast<uintptr_t>(args.D) % 8 == 0) && (reinterpret_cast<uintptr_t>(args.C) % 8 == 0);
+#pragma unroll
+      for (int j = 0; j < kBN / 8; ++j) {
+        const int col = n0 + 8 * j + 2 * (int)quad;
+        if (col >= args.N) continue;
+        const bool two = col + 1 < args.N;
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const long long grow = row0 + 8 * half;
+          if (grow >= args.M) continue;
+          float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+          float* dp = reinterpret_cast<float*>(args.D) + grow * args.ldd + col;
+          const float* cp = args.C ? reinterpret_cast<const float*>(args.C) + grow * args.ldc + col : nullptr;
+          if (two && vec) {
+            if (cp) {
+              const float2 old = *reinterpret_cast<const float2*>(cp);
+              v0 += old.x; v1 += old.y;
+            }
+            *reinterpret_cast<float2*>(dp) = make_float2(v0, v1);
+          } else {
+            dp[0] = v0 + (cp ? cp[0] : 0.f);
+            if (two) dp[1] = v1 + (cp ? cp[1] : 0.f);
+          }
+        }
+      }
+    } else {
+      const bool vec_d = (args.ldd % 8 == 0) && (reinterpret_cast<uintptr_t>(args.D) % 16 == 0);
+#pragma unroll
+      for (int g = 0; g < kBN / 32; ++g) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const long long grow = row0 + 8 * half;
+          const bool row_ok = grow < args.M;
+          uint32_t x[4];
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            const int j = 4 * g + jj;
+            const int col = n0 + 8 * j + 2 * (int)quad;
+            float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+            if (args.C != nullptr && row_ok && col < args.N) {
+              const __nv_bfloat16* cp = reinterpret_cast<const __nv_bfloat16*>(args.C) + grow * args.ldc + col;
+              v0 += __bfloat162float(cp[0]);
+              if (col + 1 < args.N) v1 += __bfloat162float(cp[1]);
+            }
+            x[jj] = pack_bf16x2(v0, v1);
+          }
+          quad_transpose(x, lane);
+          const int col = n0 + 32 * g + 8 * (int)quad;
+          if (row_ok && col < args.N)
+            store_row8(reinterpret_cast<uint16_t*>(args.D) + grow * args.ldd + col, x, args.N - col, vec_d);
+        }
+      }
+    }
   }
 }
 
@@ -291,8 +235,7 @@ static CUtensorMap make_map_2d_u8(const void* base, uint64_t rows, uint64_t cols
   return make_tensor_map(base, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-// A: [M][K] e4m3 (row pitch lda bytes), B: [N][K] e4m3; sfa / sfb: atom-tiled UE8M0 scales (see quant_mxfp8.cu:
-// sfb must hold ceil(N/128) + 1 row atoms so that a 192-row tile may read one atom past the last one).
+// A: [M][K] e4m3 (row pitch lda bytes), B: [N][K] e4m3; sfa / sfb: atom-tiled UE8M0 scales (see quant_mxfp8.cu).
 cudaError_t gemm_mxfp8(const void* A, const void* sfa, const void* B, const void* sfb, void* D, const void* C, int M,
                        int N, int K, long long lda, long long ldb, long long ldd, long long ldc, bool out_fp32,
                        int num_sms, cudaStream_t stream) {

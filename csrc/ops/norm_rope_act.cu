@@ -1,4 +1,4 @@
-// Bandwidth-bound transformer ops for sm_100a: RMSNorm (+fused residual add) fwd/bwd, RoPE fwd/bwd (in place,
+// Bandwidth-bound transformer ops for sm_90a: RMSNorm (+fused residual add) fwd/bwd, RoPE fwd/bwd (in place,
 // strided so it runs directly on the fused-QKV GEMM output), SwiGLU fwd/bwd.
 // All kernels move 16 bytes per thread per access and keep rows in registers between the reduction and the
 // normalisation pass, so each tensor is read exactly once and written exactly once.

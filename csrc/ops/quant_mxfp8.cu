@@ -123,8 +123,8 @@ quant_mxfp8_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int R, in
 
 }  // namespace
 
-// sf must hold (ceil(R/128) + 1) x (C/128 rounded up) atoms of 512 bytes, sft (ceil(C/128) + 1) x (R/128 rounded up);
-// zero-initialised by the caller (padding rows / the extra atom are read by the GEMM's B tiles).
+// sf must hold ceil(R/128) x ceil(C/128) atoms of 512 bytes, sft ceil(C/128) x ceil(R/128); zero-initialised by the
+// caller (the padding rows of the last atom are read by the GEMM's tiles).
 cudaError_t quant_mxfp8(const void* x, long long ldx, int R, int C, void* q, long long ldq, void* sf, void* qt,
                         long long ldqt, void* sft, cudaStream_t stream) {
   if (R <= 0 || C <= 0) return cudaSuccess;

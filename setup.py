@@ -16,7 +16,7 @@ class BuildWithNative(build_py):
 setup(
     name="torchacc_b200",
     version="0.1.0",
-    description="B200-native (sm_100a) training acceleration framework with TorchAcc's capabilities",
+    description="H100-native (sm_90a) training acceleration framework with TorchAcc's capabilities",
     packages=find_packages(include=["torchacc_b200", "torchacc_b200.*"]),
     package_data={"torchacc_b200": ["_C.so"]},
     python_requires=">=3.10",

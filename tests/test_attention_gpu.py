@@ -1,4 +1,4 @@
-"""tcgen05 flash-attention kernels vs the explicit fp32 reference (causal / GQA / window / varlen / packed),
+"""wgmma flash-attention kernels vs the explicit fp32 reference (causal / GQA / window / varlen / packed),
 including the cases the reference's own suite skips (SURVEY section 4: causal, local, varlen-causal)."""
 import math
 

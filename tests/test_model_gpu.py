@@ -1,4 +1,4 @@
-"""End-to-end numerics of the native Llama on the sm_100a kernels vs the PyTorch fp32 reference path."""
+"""End-to-end numerics of the native Llama on the sm_90a kernels vs the PyTorch fp32 reference path."""
 import pytest
 import torch
 

@@ -68,7 +68,7 @@ def test_symm_collectives_match_nccl():
 
 
 def test_carried_collectives_match_reference():
-    """Parameter all-gather and gradient reduce-scatter carried by tcgen05 GEMM launches (csrc/fused/carry.cuh): results
+    """Parameter all-gather and gradient reduce-scatter carried by wgmma GEMM launches (csrc/fused/carry.cuh): results
     equal the NCCL collectives, the GEMMs that carried them are still correct, the fused sum of squares matches, and
     the counters prove slices really rode inside GEMM kernels (not only in the stand-alone flush)."""
     from torchacc_b200.ops.linear import gemm

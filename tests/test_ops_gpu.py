@@ -1,4 +1,4 @@
-"""Numerics of every sm_100a kernel against a plain PyTorch fp32 reference of the same op."""
+"""Numerics of every sm_90a kernel against a plain PyTorch fp32 reference of the same op."""
 import math
 
 import pytest
@@ -324,8 +324,11 @@ def test_mxfp8_quantizer_matches_reference_and_layouts():
 
 @pytest.mark.parametrize("M,N,K", [(128, 192, 128), (256, 384, 512), (1000, 776, 384), (4096, 4096, 4096)])
 def test_mxfp8_gemm_matches_fp32_oracle(M, N, K):
-    """The tensor core applies the UE8M0 block scales itself: D must equal the fp32 product of the DEQUANTISED operands
-    (exact up to accumulation order), which pins the scale atom layout, the sf_id selection and the 192-column tiling."""
+    """The kernel applies the UE8M0 block scales when it promotes each 32-element K block: D must equal the fp32 product
+    of the DEQUANTISED operands, which pins the scale atom layout and the K-block selection (a wrong mapping is off by
+    orders of magnitude).  Hopper's e4m3 MMA adds the 32 products of a K block in a datapath that keeps about 13
+    fraction bits, so the result is not exact to fp32 rounding.  Observed on an H100, relative to the largest entry: 5.5e-5, 4.8e-5, 5.7e-5
+    and 4.6e-5 for the four shapes; the bound is 1e-4."""
     from torchacc_b200.ops import fp8
     torch.manual_seed(1)
     # per-row and per-K-block magnitudes differ by orders of magnitude: a wrong scale mapping cannot hide
@@ -337,7 +340,7 @@ def test_mxfp8_gemm_matches_fp32_oracle(M, N, K):
     d = fp8.gemm_mxfp8(aq, bq, out_dtype=torch.float32)
     ref = fp8.dequantize_mxfp8(aq).double() @ fp8.dequantize_mxfp8(bq).double().t()
     err = (d.double() - ref).abs().max() / ref.abs().max()
-    assert err < 1e-5, float(err)
+    assert err < 1e-4, float(err)
     # against the unquantised product: fp8 precision
     full = a.double() @ b.double().t()
     assert ((d.double() - full).norm() / full.norm()) < 0.06

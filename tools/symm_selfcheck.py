@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Peer-memory collectives checked against values every rank can compute locally -- NO NCCL collective in the timed /
 checked region, so the script can run under compute-sanitizer (NCCL's own kernels are not synccheck-clean and abort the
-run: profiles/sanitizer_r2.txt):
+run: the 2-GPU sanitizer run):
 
     torchrun --nproc-per-node 2 --master-addr 127.0.0.1 --no-python \
         compute-sanitizer --tool synccheck python tools/symm_selfcheck.py

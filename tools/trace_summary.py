@@ -5,7 +5,7 @@
   * time per kernel family, and how much of the communication kernels' time is hidden behind compute kernels
   * the largest idle gaps on the busiest (compute) stream with the neighbouring kernels
 
-    python tools/trace_summary.py gpurun_out/trace.json [--top 25] > profiles/step_timeline.txt
+    python tools/trace_summary.py trace.json [--top 25]
 """
 import argparse
 import gzip
@@ -18,7 +18,7 @@ COMM = ("all_gather_kernel", "reduce_scatter_kernel", "all_to_all_kernel", "mult
 
 def family(name: str) -> str:
     n = name
-    for key, fam in (("gemm_bf16_kernel", "gemm (tcgen05)"), ("flash_fwd", "attention fwd"), ("flash_bwd", "attention bwd"),
+    for key, fam in (("gemm_bf16_kernel", "gemm (wgmma)"), ("flash_fwd", "attention fwd"), ("flash_bwd", "attention bwd"),
                      ("attn_bwd_pre", "attention bwd pre/post"), ("convert", "attention bwd pre/post"),
                      ("adamw", "adamw"), ("rmsnorm", "rmsnorm"), ("rope", "rope"), ("swiglu", "swiglu"),
                      ("cross_entropy", "cross-entropy"), ("sqnorm", "grad-norm"), ("multi_copy_tma_kernel", "symm all-gather / all-to-all (TMA)"),

@@ -1,4 +1,4 @@
-"""torchacc_b200 -- a B200-native (sm_100a) training-acceleration framework with TorchAcc's capabilities.
+"""torchacc_b200 -- an H100-native (sm_90a) training-acceleration framework with TorchAcc's capabilities.
 
 ``import torchacc_b200 as ta`` provides the reference's public surface (reference torchacc/__init__.py:4-22):
 ``ta.accelerate``, ``ta.Config``, ``ta.AsyncLoader``, ``ta.amp``, ``ta.dist``, ``ta.ops``, ``ta.utils``,

@@ -105,7 +105,7 @@ def check(code: int, what: str) -> None:
 
 
 def use_native(*tensors) -> bool:
-    """Decide between the sm_100a kernels and the PyTorch reference path for these tensors."""
+    """Decide between the sm_90a kernels and the PyTorch reference path for these tensors."""
     if not tensors or not all(t.is_cuda for t in tensors if isinstance(t, torch.Tensor)):
         return False
     if os.environ.get("TORCHACC_B200_DISABLE_NATIVE", "0") == "1":   # accuracy baselines: plain PyTorch ops on the GPU
@@ -152,8 +152,8 @@ def bf16_flag(t) -> int:
 
 
 def set_gemm_scheduler(dynamic: bool) -> None:
-    """Tile scheduling of the tcgen05 GEMM: static striping (fastest when the GEMM owns the GPU) or dynamic
-    cluster-launch-control claiming (robust when collective kernels occupy some SMs on side streams).  The env
+    """Tile scheduling of the wgmma GEMM: static striping (fastest when the GEMM owns the GPU) or dynamic:
+    one CTA per tile, placed by the block scheduler (robust when collective kernels occupy some SMs on side streams).  The env
     var ``TORCHACC_B200_GEMM_SCHED=static|dynamic`` pins the mode."""
     if os.environ.get("TORCHACC_B200_GEMM_SCHED", "auto") not in ("auto", ""):
         return

@@ -4,7 +4,7 @@ Same contract as reference torchacc/accelerate.py:49-149: validate the config, b
 mesh, wrap the dataloader in an ``AsyncLoader``, apply kernel patches, build the parallel wrappers
 (PP / TP / CP / FSDP / DP), apply gradient checkpointing, move to the device and return ``model`` or
 ``(model, loader)``.  What changed underneath: no XLA flags / lazy device; kernel "patches" swap HF module
-forwards onto our sm_100a ops; deferred (meta-device) models are materialised unit by unit instead of torchdistx.
+forwards onto our sm_90a ops; deferred (meta-device) models are materialised unit by unit instead of torchdistx.
 """
 from __future__ import annotations
 
@@ -60,7 +60,7 @@ def accelerate(model: nn.Module, dataloader=None, config: Optional[Config] = Non
     from .ops import fp8 as _fp8
     if getattr(config.compute, "fp8", False):
         if device.type == "cuda" and _fp8.available():
-            _fp8.enable(True)           # linear layers: MX-FP8 (e4m3 + UE8M0 block scales) tcgen05 GEMMs, ops/fp8.py
+            _fp8.enable(True)           # linear layers: MX-FP8 (e4m3 + UE8M0 block scales) wgmma GEMMs, ops/fp8.py
         else:
             from .utils.logger import logger
             logger.warning("compute.fp8 needs a CUDA device and the native library; linear layers stay in %s",

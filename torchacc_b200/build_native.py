@@ -1,7 +1,7 @@
 """In-tree build of the native library ``torchacc_b200/_C.so``.
 
-Every ``csrc/**/*.cu`` translation unit is compiled with nvcc for sm_100a only
-(``-gencode arch=compute_100a,code=sm_100a -lineinfo``) and linked into one shared object that Python loads
+Every ``csrc/**/*.cu`` translation unit is compiled with nvcc for sm_90a only
+(``-gencode arch=compute_90a,code=sm_90a -lineinfo``) and linked into one shared object that Python loads
 with ctypes.  The kernels do not include PyTorch headers, so a full rebuild takes well under a minute and
 works on hosts without a GPU (nvcc cross-compiles).  Objects are cached by source mtime under ``build/obj``.
 """
@@ -20,7 +20,7 @@ OBJ = ROOT / "build" / "obj"
 OUT = ROOT / "torchacc_b200" / "_C.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
 ]
 
@@ -69,7 +69,7 @@ def build(verbose: bool = False, force: bool = False, jobs: int | None = None) -
             list(ex.map(compile_one, todo))
     if todo or not OUT.exists() or force:
         cmd = [nvcc, "-shared", "-o", str(OUT), *map(str, objs), "-lcudart", "-gencode",
-               "arch=compute_100a,code=sm_100a"]
+               "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

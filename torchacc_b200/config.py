@@ -8,7 +8,7 @@ Same user-facing shape as the reference ``Config`` (reference torchacc/config.py
   asserts, and every section round-trips through ``to_dict`` / ``from_dict`` / ``from_yaml`` / ``from_json``
   (the reference has a "TODO: support dict", config.py:339);
 * there is no XLA ``lazy`` backend: ``backend`` accepts ``'eager'`` (and tolerates ``'lazy'`` with a warning);
-* additions required by the B200 design: ``compute.fp8``, ``compute.fused_kernels``, ``dist.sp.mode``
+* additions required by the GPU-native design: ``compute.fp8``, ``compute.fused_kernels``, ``dist.sp.mode``
   (``ulysses`` / ``ring`` / ``2d``) and ``dist.sp.ulysses_size``, ``dist.fsdp.reduce_dtype``,
   ``dist.fsdp.fused_collectives``, ``dist.tp.sequence_parallel``; ``'sp'`` is a real mesh axis;
 * reference defects not reproduced: ``DataLoaderConfig.validate`` type-checking the wrong field
@@ -110,7 +110,7 @@ class ComputeConfig(Section):
     """fp16/bf16 mixed precision, attention replacement, kernel patches (reference config.py:27-54).
 
     New: ``fp8`` enables the block-scaled fp8 GEMM path on the linear layers of native models;
-    ``fused_kernels`` selects the hand-written sm_100a kernels for GEMM/attention/norm/rope/loss
+    ``fused_kernels`` selects the hand-written sm_90a kernels for GEMM/attention/norm/rope/loss
     (``False`` falls back to plain PyTorch ops -- the CPU plumbing tier always does).
     """
     _SPEC = {
@@ -222,13 +222,13 @@ class FSDPConfig(Section):
         # dtype of the FLAT gradient buffer: what the wgrad GEMM epilogues write, what micro-batches accumulate in and
         # what travels on the reduce-scatter wire.  "compute" (default) = bf16/fp16 buffer, fp32 accumulation at the
         # destination; "fp32" = fp32 end to end like the reference's fp32 reduce (dist/fsdp.py:204-208) at twice the
-        # gradient bytes (the wgrad GEMM accumulates into the fp32 buffer straight from tensor memory).
+        # gradient bytes (the wgrad GEMM accumulates into the fp32 buffer straight from its accumulators).
         "grad_dtype": ("compute", lambda v: v in ("compute", "fp32"), "must be 'compute' or 'fp32'"),
         "fused_collectives": (True, ) + _bool,
         "prefetch": (1, lambda v: isinstance(v, int) and v >= 0, "must be an int >= 0"),
         # None = auto: keep the gathered bf16 parameters of every unit resident from the forward through the backward
         # (one all-gather per unit and step instead of two) whenever the full bf16 copy of the model is small next to
-        # the 180 GB of HBM3e (<= 20 %); True = classic ZeRO-3 (free after forward, gather again for backward).
+        # the device memory (<= 20 %); True = classic ZeRO-3 (free after forward, gather again for backward).
         "reshard_after_forward": (None, lambda v: v is None or isinstance(v, bool), "must be None (auto) or a bool"),
     }
 

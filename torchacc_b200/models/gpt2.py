@@ -1,5 +1,5 @@
 """Native GPT-2 (the default model of the reference's benchmark, benchmarks/transformer.py:32-68 ``gpt2`` /
-``GPT2Block``): learned positions, pre-LN blocks, GELU MLP, tied embeddings.  Linear layers run on the tcgen05
+``GPT2Block``): learned positions, pre-LN blocks, GELU MLP, tied embeddings.  Linear layers run on the wgmma
 GEMM, attention on the flash kernels, the loss on fused linear + cross-entropy; LayerNorm/GELU use PyTorch ops
 (Llama-family models are the tuned path)."""
 from __future__ import annotations

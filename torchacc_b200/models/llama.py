@@ -1,4 +1,4 @@
-"""Native Llama-family decoder (Llama-2/3, Qwen2-style with QKV bias) built on the sm_100a op set.
+"""Native Llama-family decoder (Llama-2/3, Qwen2-style with QKV bias) built on the sm_90a op set.
 
 The reference has no model code of its own: it patches HF models (liger kernels, FA) and relies on FlashModels
 for TP/CP-aware modules (SURVEY 2.1 #27, #41, 7.1 "native Llama model definition").  This module is that native

@@ -1,4 +1,4 @@
-"""FlashAttention API on the hand-written tcgen05 kernels (csrc/attn/).
+"""FlashAttention API on the hand-written wgmma kernels (csrc/attn/).
 
 Public functions keep the reference signatures (reference torchacc/ops/flash_attn.py:313-601): layout
 ``[B, S, H, D]``, ``softmax_scale``, ``causal`` (bottom-right aligned), ``window_size=(left, right)``,
@@ -7,8 +7,8 @@ aliases.  Variants: fixed length, padded batch + ``attention_mask`` (varlen), pa
 ``position_ids == 0``, and QKV-packed.
 
 Backends (``set_attention_backend``):
-  * ``"native"``  -- sm_100a kernels: S=QK^T and O+=PV on tcgen05 with TMEM accumulators, TMA-fed K/V ring,
-                     online softmax in registers; backward with five tcgen05 GEMMs per tile.
+  * ``"native"``  -- sm_90a kernels: S=QK^T and O+=PV on wgmma with register accumulators, TMA-fed K/V ring,
+                     online softmax in registers; backward with five wgmma GEMMs per tile.
   * ``"sdpa"``    -- ``torch.nn.functional.scaled_dot_product_attention`` (library; bring-up / unsupported shapes)
   * ``"reference"`` -- explicit fp32 math (test oracle; the only backend on CPU).
 Features the native kernels do not cover (dropout > 0, ALiBi, head_dim not in {64, 128}) route to ``sdpa`` /

@@ -385,8 +385,7 @@ def _masked_diag(q, k, v, scale, lens):
 class _LazyRing:
     """Classic ring exchange with the NEXT transfer always in flight: block ``(rank - s) % cp`` arrives in round ``s``, and
     as soon as the consumer asks for it the block is forwarded to the next rank, so that transfer overlaps the consumer's
-    attention on the block (the reference overlaps the same way with its RingComm, context_parallel/utils.py:398-415;
-    round 1 of this file waited for every transfer before computing anything)."""
+    attention on the block (the reference overlaps the same way with its RingComm, context_parallel/utils.py:398-415)."""
 
     def __init__(self, kv: torch.Tensor, group):
         self.group = group

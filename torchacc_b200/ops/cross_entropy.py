@@ -1,7 +1,7 @@
 """Cross-entropy and fused linear + cross-entropy.
 
 ``fused_linear_cross_entropy(hidden, lm_head_weight, labels)`` never materialises the ``[T, V]`` logits for the
-whole batch: tokens are processed in chunks; for each chunk the lm_head GEMM (tcgen05) produces bf16 logits, the
+whole batch: tokens are processed in chunks; for each chunk the lm_head GEMM (wgmma) produces bf16 logits, the
 CE kernel (csrc/ops/loss_optim.cu) computes the row losses and overwrites the logits with their gradient, and the
 dgrad / wgrad GEMMs consume that gradient immediately (wgrad accumulates across chunks in the GEMM epilogue).
 Same idea as liger's fused-linear-CE that the reference enables by default

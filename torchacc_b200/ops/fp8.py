@@ -1,7 +1,7 @@
-"""Block-scaled FP8 (MX: e4m3 + one UE8M0 scale per 32 elements) linear layers on tcgen05
+"""Block-scaled FP8 (MX: e4m3 + one UE8M0 scale per 32 elements) linear layers on wgmma
 (csrc/gemm/gemm_mxfp8.cu, csrc/ops/quant_mxfp8.cu).  Enabled by ``Config.compute.fp8``.
 
-All three GEMMs of a linear layer run in fp8 with fp32 accumulation in tensor memory:
+All three GEMMs of a linear layer run in fp8 with fp32 accumulation in registers:
 
     forward  y  = x  W^T : x  quantised along features,   W   along in-features
     dgrad    dx = dy W   : dy quantised along out-features, W^T along out-features   (transposed quantisation of W)
@@ -56,7 +56,7 @@ class MXTensor:
 
 
 def _sf_buffer(rows: int, k: int, device) -> torch.Tensor:
-    atoms_r = (rows + ATOM_ROWS - 1) // ATOM_ROWS + 1          # + 1: a 192-row GEMM tile may read one atom further
+    atoms_r = (rows + ATOM_ROWS - 1) // ATOM_ROWS
     atoms_k = (k + ATOM_K - 1) // ATOM_K
     return torch.zeros(atoms_r * atoms_k * 512, dtype=torch.uint8, device=device)
 

@@ -2,7 +2,7 @@
 
 The reference swaps HF module forwards onto liger's Triton kernels.  Same entry points here
 (``apply_liger_kernel``, ``apply_liger_kernel_to_llama``, ``apply_liger_kernel_to_qwen2``) but the replacements are
-our sm_100a kernels: RMSNorm, SwiGLU, RoPE-free fused loss (linear + cross-entropy), and the tcgen05 GEMM behind
+our sm_90a kernels: RMSNorm, SwiGLU, RoPE-free fused loss (linear + cross-entropy), and the wgmma GEMM behind
 every ``nn.Linear`` of the model.  Patches are applied to *classes* (like liger) or to one model instance.
 """
 from __future__ import annotations
@@ -135,7 +135,7 @@ def _patch_rope(modeling) -> None:
 
 
 def patch_linears(model: nn.Module) -> int:
-    """Route every ``nn.Linear`` of this model instance through the tcgen05 GEMM."""
+    """Route every ``nn.Linear`` of this model instance through the wgmma GEMM."""
     n = 0
     for m in model.modules():
         if type(m) is nn.Linear:
@@ -166,7 +166,7 @@ def apply_liger_kernel(model: Optional[nn.Module] = None) -> None:
             except Exception as e:  # pragma: no cover - depends on the installed transformers
                 logger.debug("kernel patch %s skipped: %s", fn.__name__, e)
         if wanted:
-            # HF attention call sites (flash_attention_2 / the attention-interface registry) -> our tcgen05 kernels; the
+            # HF attention call sites (flash_attention_2 / the attention-interface registry) -> our wgmma kernels; the
             # reference does this at import time (torchacc/__init__.py:135), here it happens when a model needs it
             from ..utils.patch import patch_fa
             patch_fa()

@@ -1,4 +1,4 @@
-"""Linear layers on the hand-written tcgen05 GEMM (csrc/gemm/gemm_bf16.cu).
+"""Linear layers on the hand-written wgmma GEMM (csrc/gemm/gemm_bf16.cu).
 
 ``linear(x, w, bias)`` computes ``x @ w.T + bias`` with three launches of the same kernel:
 forward (K-major/K-major), dgrad (K-major/MN-major) and wgrad (MN-major/MN-major) -- no transposed copies.
@@ -10,7 +10,6 @@ The reference reaches cuBLAS through ``nn.Linear`` here (SURVEY 2.4a "Dense GEMM
 """
 from __future__ import annotations
 
-import os
 from typing import Optional
 
 import torch
@@ -18,7 +17,7 @@ import torch.nn.functional as F
 
 from .. import _native as nat
 
-_CLUSTER = int(os.environ.get("TORCHACC_B200_GEMM_CLUSTER", "2"))
+_CLUSTER = 1   # CTA-pair tiles do not exist on sm_90a; the C ABI keeps the argument
 
 
 def gemm(a: torch.Tensor, b: torch.Tensor, *, a_mn_major: bool = False, b_mn_major: bool = False,
@@ -136,7 +135,7 @@ class _LinearFn(torch.autograd.Function):
 
 def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
            residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """Drop-in for ``F.linear`` (bf16 CUDA tensors go through the tcgen05 GEMM).  ``residual`` (same shape as the
+    """Drop-in for ``F.linear`` (bf16 CUDA tensors go through the wgmma GEMM).  ``residual`` (same shape as the
     result) is added inside the GEMM epilogue: ``x @ w.T + bias + residual`` without a separate elementwise pass."""
     if x.is_cuda and nat.is_half(x, w) and nat.use_native(x, w):
         from . import fp8
@@ -148,7 +147,7 @@ def linear(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None
 
 
 class Linear(torch.nn.Linear):
-    """``nn.Linear`` whose forward/backward run on the tcgen05 GEMM."""
+    """``nn.Linear`` whose forward/backward run on the wgmma GEMM."""
 
     def forward(self, x):
         return linear(x, self.weight, self.bias)

@@ -1,4 +1,4 @@
-"""RMSNorm (+ fused residual add) on the sm_100a kernels in csrc/ops/norm_rope_act.cu.
+"""RMSNorm (+ fused residual add) on the sm_90a kernels in csrc/ops/norm_rope_act.cu.
 
 Replaces liger's Triton RMSNorm that the reference patches into HF Llama/Qwen2
 (reference torchacc/ops/liger.py:10-18).  Semantics follow HF ``LlamaRMSNorm``: statistics in fp32,

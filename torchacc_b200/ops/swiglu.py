@@ -114,7 +114,7 @@ nat.register_signatures({
 
 
 class _GateUpSwiGLUFn(torch.autograd.Function):
-    """h = silu(x Wg^T) * (x Wu^T) in ONE tcgen05 GEMM (csrc/gemm/gemm_bf16.cu, SwiGLU epilogue: the CTA pair stages the
+    """h = silu(x Wg^T) * (x Wu^T) in ONE wgmma GEMM (csrc/gemm/gemm_bf16.cu, SwiGLU epilogue: every stage holds the
     matching gate / up weight rows, so both halves of an output column sit in the same accumulator tile)."""
 
     @staticmethod

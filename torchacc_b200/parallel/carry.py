@@ -1,7 +1,7 @@
 """Collectives carried inside the GEMM kernels (csrc/fused/carry.cuh / carry.cu) -- the FSDP hot path.
 
 Instead of launching the parameter all-gather and the gradient reduce-scatter of a unit as their own kernels on side
-streams, the sharding engine *enqueues* them here.  Every tcgen05 GEMM launched afterwards (forward, recomputation,
+streams, the sharding engine *enqueues* them here.  Every wgmma GEMM launched afterwards (forward, recomputation,
 dgrad, wgrad, the chunked lm_head) takes a slice of the pending jobs proportional to its FLOPs, and warp 3 of each of
 its CTAs moves that slice over NVLink with TMA bulk copies while the tile pipeline of the same CTA runs:
 
@@ -181,9 +181,7 @@ def make_carry(coll, device: torch.device) -> Optional[CarryRuntime]:
     if mode == "0":
         return None
     if mode == "auto" and coll.domain.world > 2:
-        # measured (profiles/carry_n8_r2.txt): carried collectives win at 2 GPUs (502-507 vs 510-512 ms / step) and
-        # lose at 8 (528-565 vs 511-515 ms): with 8 ranks a reduce stage is eight 1 KB bulk loads and every GEMM CTA's
-        # copy warp fans in from 7 peers.  Until the copy role uses larger per-peer stages the stand-alone TMA
+        # with 8 ranks a reduce stage is eight 1 KB bulk loads and every GEMM CTA's copy warp fans in from 7 peers.  Until the copy role uses larger per-peer stages the stand-alone TMA
         # collectives (side streams, communication windows) stay the default beyond 2 ranks; TORCHACC_B200_CARRY=1 forces it.
         return None
     return CarryRuntime(coll, device)

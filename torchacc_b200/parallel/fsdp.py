@@ -14,10 +14,9 @@ dist/dp.py:20-89 (torch DDP).  This is our own runtime, not a wrapper:
 * schedule: all-gathers are prefetched one unit ahead on a high-priority communication stream, reduce-scatters run
   on a second one behind the backward; on a GPU both are *queued* at unit boundaries and *started* at the next
   communication window (the MLP of the running / recomputed layer, ``ShardingEngine.comm_window``) so they overlap
-  large GEMMs instead of flash-attention and the small projections; the tcgen05 GEMM switches to dynamic
-  (cluster-launch-control) tile claiming while collectives share the GPU.  Gather / gradient buffers come from small
-  rotating pools so memory stays at ``2 units`` regardless of depth (sized for 180 GB HBM: Llama-3-8B on one GPU keeps
-  everything resident);
+  large GEMMs instead of flash-attention and the small projections; the wgmma GEMM switches to dynamic
+  scheduling (one CTA per tile) while collectives share the GPU.  Gather / gradient buffers come from small
+  rotating pools so memory stays at ``2 units`` regardless of depth;
 * strategies: ``FULL_SHARD`` (fsdp), ``HYBRID`` (fsdp x dp replicas), ``NO_SHARD`` (pure DP: units act as
   gradient all-reduce buckets overlapped with backward -- this is the DataParallel engine);
 * gradient checkpointing (``gc``) happens INSIDE the unit, so recomputation reuses the gathered parameters
@@ -574,7 +573,7 @@ class ShardingEngine:
         # keep_gathered: parameters stay sharded (ZeRO-3 memory for master weights / optimizer state / gradients) but
         # the gathered compute copy of every unit lives in its own persistent buffer from the forward until the end
         # of the backward -- one all-gather per unit and step instead of two.  Auto: on when that full copy is at most
-        # 20 % of the device memory (Llama-3-8B: 16 GB of 180 GB); a 70 B model falls back to re-gathering.
+        # 20 % of the device memory; a 70 B model falls back to re-gathering.
         self.keep_gathered = False
         if self.reshard:
             if reshard_after_forward is None:
@@ -626,8 +625,8 @@ class ShardingEngine:
             nat.set_gemm_scheduler(self.carry is None)
         # communication windows: on a GPU the flash-attention CTAs need whole SMs (224 KB smem) and small GEMMs are
         # the most sensitive to a concurrent collective, so prefetch all-gathers and gradient reduce-scatters are
-        # not started at unit boundaries but at the next "window" = the start of an MLP, where ~2-5 ms of large GEMMs
-        # follow (measured: profiles/step_timeline_n8_run26.txt).  TORCHACC_B200_COMM_WINDOWS=0 restores the old timing.
+        # not started at unit boundaries but at the next "window" = the start of an MLP, where the large GEMMs
+        # follow.  TORCHACC_B200_COMM_WINDOWS=0 restores the old timing.
         import os as _os
         _cw = _os.environ.get("TORCHACC_B200_COMM_WINDOWS", "1")           # "0" off, "force" also on CPU (tests)
         self.comm_windows = bool(self.world_data > 1 and (_cw == "force" or (cuda and _cw != "0")))
@@ -636,7 +635,6 @@ class ShardingEngine:
         # optional "head" unit (final norm + lm_head split off the root unit, TORCHACC_B200_SPLIT_HEAD=1): its
         # gradients are complete right after the loss backward, so its reduce-scatter hides behind the whole
         # backward pass instead of sitting exposed before the optimizer with the embedding's
-        # default on since round 2 (2 GPUs: exposed communication 6.9 -> 3.8 ms per step, profiles/split_head_n2_r2.txt)
         self.split_head = _os.environ.get("TORCHACC_B200_SPLIT_HEAD", "1") == "1"
         self.head_unit: Optional[FlatParamUnit] = None
         self._head_staged = False

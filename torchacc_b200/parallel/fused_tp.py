@@ -82,7 +82,7 @@ class FusedTP:
         d = self.domain
         buf = d.find(full)
         # copy clusters: a short GEMM (small N) has little math to hide the transfer behind -> more copy CTAs;
-        # a long one prefers the SMs for tensor work (measured at N=2: profiles/fused_tp_bench_*.txt)
+        # a long one prefers the SMs for tensor work
         cc = self.comm_clusters if self.comm_clusters > 0 else (8 if N <= 4096 else 4)
         self.flag_total = getattr(self, "flag_total", 0) + cc * 2
         self.flag_calls += 1
@@ -106,14 +106,14 @@ class FusedTP:
         N = w.shape[1] if b_mn_major else w.shape[0]
         rows = M // self.world
         key = (rows, N)
-        slot = rows * ((N + 255) // 256 * 256)       # block-major slots, N padded to the 256-column tile
+        slot = rows * ((N + 255) // 256 * 256)       # row-major slots, N padded to the 256-column tile
         if key not in self._stage:
             self._stage[key] = self.domain.alloc(self.world * slot, torch.bfloat16)
         stage = self._stage[key]
         d = self.domain
         sbuf, cbuf = d.find(stage), d.find(self.counters)
-        tiles = (rows // TILE_M) * ((N + 255) // 256)
-        self.counter_expected += tiles * 8          # 2 CTAs x 4 epilogue warps per 256-row tile
+        tiles = (rows // 128) * ((N + 255) // 256)
+        self.counter_expected += tiles * 8          # 2 MMA warpgroups x 4 warps per 128-row tile
         L = nat.require()
         nat.check(
             L.tb_gemm_rs_bf16(x.data_ptr(), w.data_ptr(), sbuf.peer_ptrs, cbuf.peer_ptrs, d.pad_ptrs, rows, N, K,

@@ -112,7 +112,7 @@ class StageLink:
         send/recv for the same reason).  NCCL creates a communicator / p2p channel at its first use with a host-side
         rendezvous of both peers; inside the 1F1B schedule the two stages reach their first gradient transfer at
         different points, and the stage that arrives first blocks on the host while its neighbour's device sits in an
-        early-posted receive that only the blocked stage could satisfy (observed on 2 B200: profiles/pp_hang_r2.txt).
+        early-posted receive that only the blocked stage could satisfy.
         One tiny exchange per direction and communicator, in the same order on every stage, then a device sync."""
         if self.stages <= 1 or not (dist.is_available() and dist.is_initialized()):
             return

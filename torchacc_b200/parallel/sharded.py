@@ -24,8 +24,7 @@ class _AutocastModel(nn.Module):
         self.model = model
         self.dtype, self.device_type = dtype, device_type
         # intermediate pipeline stages hand their activations to the next stage in the compute dtype: converting them
-        # to fp32 doubled the p2p bytes AND pushed the next stage onto the non-native fp32 fallback ops (found on 2
-        # B200 in round 2: profiles/pp_gpu_r2.txt)
+        # to fp32 doubled the p2p bytes AND pushed the next stage onto the non-native fp32 fallback ops
         self.fp32_outputs = fp32_outputs
 
     def __getattr__(self, name):

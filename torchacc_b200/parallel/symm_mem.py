@@ -40,7 +40,7 @@ nat.register_signatures({
 # the k-th further SymmCollectives instance.  The device protocol requires the collectives of ONE channel to run in the
 # same order on every rank; two users that issue from different streams (the engine's gradient all-reduce on its
 # reduce stream, ring attention's reduce-scatter on the compute stream) therefore get their own channel block
-# (found with the bounded spins on 8 GPUs in round 2: profiles/ring_cp8_deadlock_r2.txt).
+# (found with the bounded spins on 8 GPUs).
 CH_ALL_GATHER, CH_REDUCE_SCATTER, CH_ALL_REDUCE, CH_ALL_TO_ALL, CH_USER0 = 0, 1, 2, 3, 8
 _FIRST_EXTRA_BLOCK, _MAX_BLOCKS = 16, 12
 _PAD_BYTES = 64 * 16 * 4

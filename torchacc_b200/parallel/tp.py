@@ -83,7 +83,7 @@ class _ColumnParallel(torch.autograd.Function):
         x2 = x.reshape(-1, x.shape[-1])
         f = tp.fused
         if tp.sequence_parallel and f is not None and x2.is_cuda and f.ok_ag(x2.shape[0], w.shape[0], x2.shape[1], x2.dtype):
-            y, _ = f.ag_gemm(x2.contiguous(), w, bias)          # ONE kernel: peer pull of the token shards + tcgen05 GEMM
+            y, _ = f.ag_gemm(x2.contiguous(), w, bias)          # ONE kernel: peer pull of the token shards + wgmma GEMM
         else:
             xf = _all_gather_rows(x2, tp) if tp.sequence_parallel else x2
             y = _mm(xf, w, bias=bias, out_dtype=x.dtype)

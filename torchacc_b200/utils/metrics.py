@@ -5,7 +5,7 @@ SURVEY 5.5).
 * ``ThroughputMeter``: CUDA-event timing of a window of steps, reduced with MAX over ranks (the number a whole job
   actually achieves), host wall-clock fallback on CPU.
 * ``memory_stats()``: allocator + engine view of device memory in GB (what is resident: master/compute shards,
-  gradient shards, pooled gather/gradient buffers) -- sized against the 180 GB of a B200.
+  gradient shards, pooled gather/gradient buffers).
 """
 from __future__ import annotations
 
