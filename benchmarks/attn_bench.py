@@ -1,7 +1,9 @@
 """Attention micro-benchmark: our wgmma kernels vs the library paths (torch SDPA / flash-attn 2) on the Llama-3-8B
-attention shape.  CUDA-event timing, L2 flushed between iterations."""
+attention shape.  CUDA-event timing, L2 flushed between iterations.  ``--deterministic`` also times the deterministic
+backward (atomic-free dQ kernel) in the same run; the card name and power limit are reported with the numbers."""
 import argparse
 import json
+import subprocess
 import sys
 import os
 
@@ -26,6 +28,18 @@ def timeit(fn, iters=10, warmup=3):
     return min(ts), sum(ts) / len(ts)
 
 
+def device_desc():
+    """Card name and power limit (W) of cuda:0, read with nvidia-smi when it is available."""
+    desc = {"gpu": torch.cuda.get_device_name(0)}
+    try:
+        r = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=30)
+        desc["power_limit_w"] = float(r.stdout.strip().splitlines()[0])
+    except Exception:
+        desc["power_limit_w"] = None
+    return desc
+
+
 def main():
     p = argparse.ArgumentParser()
     p.add_argument("--batch", type=int, default=2)
@@ -34,6 +48,8 @@ def main():
     p.add_argument("--hk", type=int, default=8)
     p.add_argument("--d", type=int, default=128)
     p.add_argument("--only", default="", help="native: skip the library paths")
+    p.add_argument("--deterministic", action="store_true",
+                   help="also time the native deterministic backward (deterministic=True)")
     a = p.parse_args()
     from torchacc_b200.ops import attention as A
     B, S, Hq, Hk, D = a.batch, a.seq, a.hq, a.hk, a.d
@@ -59,8 +75,11 @@ def main():
 
     A.set_attention_backend("native")
     bench("tb_native", lambda: A.flash_attn_func(q, k, v, causal=True))
+    if a.deterministic:
+        bench("tb_native_deterministic", lambda: A.flash_attn_func(q, k, v, causal=True, deterministic=True))
+    dev_desc = device_desc()
     if a.only == "native":
-        print(json.dumps({"shape": [B, S, Hq, Hk, D], "results": res}))
+        print(json.dumps({"shape": [B, S, Hq, Hk, D], "device": dev_desc, "results": res}))
         return
     A.set_attention_backend("sdpa")
     bench("torch_sdpa", lambda: A.flash_attn_func(q, k, v, causal=True))
@@ -69,7 +88,7 @@ def main():
         bench("flash_attn2", lambda: fa2(q, k, v, causal=True))
     except Exception as e:
         print("flash_attn unavailable:", e)
-    print(json.dumps({"shape": [B, S, Hq, Hk, D], "results": res}))
+    print(json.dumps({"shape": [B, S, Hq, Hk, D], "device": dev_desc, "results": res}))
 
 
 if __name__ == "__main__":

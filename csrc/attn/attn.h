@@ -28,13 +28,16 @@ cudaError_t flash_attn_fwd_ex(const void* q, const void* k, const void* v, void*
 
 // Blockwise backward: phases bit 0 = preprocess (delta = rowsum(dO o O), dq_acc = 0), bit 1 = main kernel (dK/dV of the
 // visited keys, dQ reduce-added into dq_acc), bit 2 = dq = cast(dq_acc).  A ring step runs bit 1 only.
+// deterministic: bit 0 computes delta only, bit 1 computes dK/dV only, bit 2 runs the query-stationary dQ kernel, which
+// writes dq directly without atomics (bitwise reproducible; dq_acc is not used and may be null).
 cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const void* o, const void* dout,
                               const float* lse, void* dq, void* dk, void* dv, float* dq_acc, float* delta,
                               const int* cu_q, const int* cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
                               long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale, bool causal,
                               int wl, int wr, long long Tq, long long Tk, long long dq_ts, long long dk_ts,
                               long long dv_ts, int num_sms, bool is_bf16, const float* alibi_slopes,
-                              int alibi_batch_stride, BlockView view, int phases, cudaStream_t stream);
+                              int alibi_batch_stride, BlockView view, int phases, cudaStream_t stream,
+                              bool deterministic = false);
 
 cudaError_t flash_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_q,
                            const int* cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts,

@@ -21,6 +21,7 @@
 #include "../common/tensormap.h"
 #include "attn.h"
 #include "dropout.cuh"
+#include "mask.cuh"
 
 namespace tb {
 
@@ -65,15 +66,6 @@ struct FwdSmem {
   static constexpr int kTotal = kBar + 256 + 1024;
 };
 
-// visible key range [lo, hi] for query row `row` (0-based inside its sequence)
-__device__ __forceinline__ void key_bounds(int row, int q_len, int k_len, int causal, int wl, int wr, int& lo, int& hi) {
-  const int pos = row + (k_len - q_len);
-  int r = wr;
-  if (causal) r = (wr < 0) ? 0 : min(wr, 0);
-  hi = (r < 0) ? (k_len - 1) : min(k_len - 1, pos + r);
-  lo = (wl < 0) ? 0 : max(0, pos - wl);
-}
-
 template <int D, bool kBf16, bool kDrop>
 __global__ void __launch_bounds__(kFwdThreads, 1)
 flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
@@ -95,14 +87,8 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const bool merging = args.acc != nullptr;
 
   // KV tile range touched by this query tile
-  int lo_first, hi_first, lo_last, hi_last;
-  const int last_row = min(m0 + kBM, q_len) - 1;
-  key_bounds(m0, q_len, k_len, args.causal, args.wl, args.wr, lo_first, hi_first);
-  key_bounds(last_row, q_len, k_len, args.causal, args.wl, args.wr, lo_last, hi_last);
-  const int kmin = lo_first, kmax = hi_last;
-  const int j_lo = kmin / kBN;
-  const int j_hi = (kmax < 0 || kmax < kmin) ? j_lo : (kmax / kBN + 1);
-  const int n_tiles = j_hi - j_lo;
+  int j_lo, n_tiles;
+  key_tile_range(m0, kBM, q_len, k_len, args.causal, args.wl, args.wr, kBN, j_lo, n_tiles);
 
   if (n_tiles <= 0) {  // nothing visible: O = 0, LSE = -inf (merging: the running result is unchanged)
     for (int r = threadIdx.x; r < min(kBM, q_len - m0); r += blockDim.x) {
@@ -224,19 +210,7 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     if (tracing && t < 64) args.trace[t * 16 + 1] = clock64();
 
     // ---- scale / mask / online softmax ----
-    const bool interior = !has_alibi && n0 >= lo[0] && n0 >= lo[1] && n0 + kBN - 1 <= hi[0] && n0 + kBN - 1 <= hi[1];
-    if (!__all_sync(0xffffffffu, interior)) {
-#pragma unroll
-      for (int j = 0; j < kBN / 8; ++j)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int i = e >> 1;
-          const int kidx = n0 + 8 * j + 2 * (int)quad + (e & 1);
-          float v = sacc[4 * j + e];
-          if (has_alibi) v = fmaf(v, args.scale_log2, -slope_l2 * fabsf((float)(pos_q[i] - kidx)));
-          sacc[4 * j + e] = (kidx >= lo[i] && kidx <= hi[i]) ? v : -INFINITY;
-        }
-    }
+    mask_score_tile<kBN>(sacc, n0, quad, lo, hi, pos_q, has_alibi, args.scale_log2, slope_l2);
     float alpha[2], mref[2], psum[2] = {0.f, 0.f};
 #pragma unroll
     for (int i = 0; i < 2; ++i) {

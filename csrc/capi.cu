@@ -94,6 +94,11 @@ TB_API int tb_sqnorm_accumulate(uint64_t g, int is_bf16, long long n, uint64_t o
                                 uint64_t stream) {
   return (int)tb::sqnorm_accumulate(P<void>(g), is_bf16 != 0, n, P<float>(out), pre_scale, num_sms, S(stream));
 }
+TB_API int tb_sqnorm_accumulate_ordered(uint64_t g, int is_bf16, long long n, uint64_t out, float pre_scale,
+                                        uint64_t partial, uint64_t counter, int num_sms, uint64_t stream) {
+  return (int)tb::sqnorm_accumulate_ordered(P<void>(g), is_bf16 != 0, n, P<float>(out), pre_scale, P<float>(partial),
+                                            P<unsigned int>(counter), num_sms, S(stream));
+}
 TB_API int tb_scale_inplace(uint64_t g, int is_bf16, long long n, uint64_t scale, int num_sms, uint64_t stream) {
   return (int)tb::scale_inplace(P<void>(g), is_bf16 != 0, n, P<float>(scale), num_sms, S(stream));
 }
@@ -150,6 +155,25 @@ TB_API int tb_flash_attn_bwd_dropout(uint64_t q, uint64_t k, uint64_t v, uint64_
                                     P<int>(cu_q), P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, do_ts, scale,
                                     causal != 0, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16 != 0,
                                     P<float>(alibi), alibi_bs, view, 7, S(stream));
+}
+
+// Deterministic backward: the dropout variant's arguments (p_drop = 0: no dropout).  dK/dV come from the main kernel
+// without its dQ step, dQ from the query-stationary dQ kernel; no atomics, so repeated calls are bitwise equal.
+// dq_acc is unused.
+TB_API int tb_flash_attn_bwd_deterministic(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t dout, uint64_t lse,
+                                           uint64_t dq, uint64_t dk, uint64_t dv, uint64_t dq_acc, uint64_t delta,
+                                           uint64_t cu_q, uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
+                                           long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale,
+                                           int causal, int wl, int wr, long long Tq, long long Tk, long long dq_ts,
+                                           long long dk_ts, long long dv_ts, int num_sms, uint64_t stream, int is_bf16,
+                                           uint64_t alibi, int alibi_bs, float p_drop, uint64_t seed) {
+  tb::BlockView view;
+  view.p_drop = p_drop; view.seed = seed;
+  return (int)tb::flash_attn_bwd_ex(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<void>(dout), P<float>(lse),
+                                    P<void>(dq), P<void>(dk), P<void>(dv), P<float>(dq_acc), P<float>(delta),
+                                    P<int>(cu_q), P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, do_ts, scale,
+                                    causal != 0, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16 != 0,
+                                    P<float>(alibi), alibi_bs, view, 7, S(stream), /*deterministic=*/true);
 }
 
 // Blockwise (ring) variants: BlockView addressing + in-kernel (out, lse) merge / phased backward (csrc/attn/attn.h).

@@ -253,6 +253,72 @@ cudaError_t sqnorm_accumulate(const void* g, bool is_bf16, long long n, float* o
   return cudaGetLastError();
 }
 
+// Deterministic variant, still one launch: every block writes its partial sum to partial[blockIdx.x] and takes an
+// integer ticket; the last block to finish adds the partials in index order to out[0] and resets the counter.  Only the
+// ticket order depends on scheduling, never a value, and the grid depends on n and the SM count only, so repeated
+// calls give bitwise-equal sums.  found_inf is the same idempotent flag write as in sqnorm_kernel.
+template <typename GradT>
+__global__ void __launch_bounds__(256)
+sqnorm_ordered_kernel(const GradT* __restrict__ g, long long n, float* __restrict__ out, float pre_scale,
+                      float* __restrict__ partial, unsigned int* __restrict__ counter) {
+  __shared__ float red[8];
+  __shared__ bool last;
+  float acc = 0.f;
+  bool bad = false;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n;
+       i += (long long)gridDim.x * blockDim.x) {
+    float x;
+    if constexpr (sizeof(GradT) == 4) x = g[i]; else x = __bfloat162float(g[i]);
+    x *= pre_scale;
+    bad |= !isfinite(x);
+    acc += x * x;
+  }
+  acc = warp_reduce_sum(acc);
+  const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) red[w] = acc;
+  const int any_bad = __syncthreads_or(bad ? 1 : 0);
+  if (w == 0) {
+    float t = l < 8 ? red[l] : 0.f;
+    t = warp_reduce_sum(t);
+    if (l == 0) {
+      partial[blockIdx.x] = t;
+      if (any_bad) out[1] = 1.f;
+      __threadfence();                                   // the partial is visible before the ticket is taken
+      last = atomicAdd(counter, 1u) == gridDim.x - 1;
+    }
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  // fixed-shape reduction over the partials: thread t sums t, t + 256, ... in order, then the block tree
+  float s = 0.f;
+  for (int i = threadIdx.x; i < (int)gridDim.x; i += blockDim.x) s += __ldcg(partial + i);
+  s = warp_reduce_sum(s);
+  if (l == 0) red[w] = s;
+  __syncthreads();
+  if (w == 0) {
+    float t = l < 8 ? red[l] : 0.f;
+    t = warp_reduce_sum(t);
+    if (l == 0) {
+      out[0] += t;
+      *counter = 0u;                                     // ready for the next launch on this stream
+    }
+  }
+}
+
+cudaError_t sqnorm_accumulate_ordered(const void* g, bool is_bf16, long long n, float* out, float pre_scale,
+                                      float* partial, unsigned int* counter, int num_sms, cudaStream_t stream) {
+  if (n == 0) return cudaSuccess;
+  long long blocks = (n + 256 * 8 - 1) / (256 * 8);     // same grid as sqnorm_accumulate: at most 8 blocks per SM
+  int grid = (int)(blocks < (long long)num_sms * 8 ? blocks : (long long)num_sms * 8);
+  if (is_bf16)
+    sqnorm_ordered_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>((const __nv_bfloat16*)g, n, out, pre_scale, partial,
+                                                                   counter);
+  else
+    sqnorm_ordered_kernel<float><<<grid, 256, 0, stream>>>((const float*)g, n, out, pre_scale, partial, counter);
+  return cudaGetLastError();
+}
+
 // g *= *scale (in place) -- GradScaler unscale / clip for optimizers that are not ours.
 template <typename GradT>
 __global__ void __launch_bounds__(256) scale_kernel(GradT* __restrict__ g, long long n, const float* __restrict__ scale) {

@@ -26,6 +26,10 @@ cudaError_t adamw_flat(float* p, const void* g, bool grad_is_bf16, float* m, flo
                        const float* grad_scale, const float* found_inf, int num_sms, cudaStream_t stream);
 cudaError_t sqnorm_accumulate(const void* g, bool is_bf16, long long n, float* out, float pre_scale, int num_sms,
                               cudaStream_t stream);
+// Same sums in a fixed order (bitwise reproducible), one launch: partial = fp32 workspace of >= 8 * num_sms floats,
+// counter = one zeroed uint32 that the launch leaves zeroed again; launches sharing them must be stream-ordered.
+cudaError_t sqnorm_accumulate_ordered(const void* g, bool is_bf16, long long n, float* out, float pre_scale,
+                                      float* partial, unsigned int* counter, int num_sms, cudaStream_t stream);
 // MX-FP8 quantiser (ops/quant_mxfp8.cu): row-wise (q, sf) and / or transposed (qt, sft) e4m3 + UE8M0 outputs of a bf16
 // matrix x[R][C]; either pair may be null.
 cudaError_t quant_mxfp8(const void* x, long long ldx, int R, int C, void* q, long long ldq, void* sf, void* qt,

@@ -67,6 +67,10 @@ def accelerate(model: nn.Module, dataloader=None, config: Optional[Config] = Non
                            "bf16" if config.compute.bf16 else "fp32")
     else:
         _fp8.enable(False)
+    # deterministic mode: atomic-free attention dQ and ordered gradient-norm sums (process-wide, like compute.fp8)
+    from .ops import attention as _attn, optim as _optim
+    _attn.set_deterministic(config.compute.deterministic)
+    _optim.set_deterministic(config.compute.deterministic)
     if config.compute.acc_scaled_dot_attn:
         from .ops.sdpa import patch_sdpa
         patch_sdpa()

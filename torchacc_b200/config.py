@@ -111,7 +111,9 @@ class ComputeConfig(Section):
 
     New: ``fp8`` enables the block-scaled fp8 GEMM path on the linear layers of native models;
     ``fused_kernels`` selects the hand-written sm_90a kernels for GEMM/attention/norm/rope/loss
-    (``False`` falls back to plain PyTorch ops -- the CPU plumbing tier always does).
+    (``False`` falls back to plain PyTorch ops -- the CPU plumbing tier always does);
+    ``deterministic`` makes a single-GPU training step bitwise reproducible: the attention backward computes dQ
+    without atomics and the gradient-norm reduction sums in a fixed order (off by default).
     """
     _SPEC = {
         "fp16": (False, ) + _bool,
@@ -120,6 +122,7 @@ class ComputeConfig(Section):
         "acc_scaled_dot_attn": (False, ) + _bool,
         "disable_kernel_patches": (False, ) + _bool,
         "fused_kernels": (True, ) + _bool,
+        "deterministic": (False, ) + _bool,
     }
 
     def _cross_validate(self):

@@ -11,6 +11,9 @@ Backends (``set_attention_backend``):
                      online softmax in registers; backward with five wgmma GEMMs per tile.
   * ``"sdpa"``    -- ``torch.nn.functional.scaled_dot_product_attention`` (library; bring-up / unsupported shapes)
   * ``"reference"`` -- explicit fp32 math (test oracle; the only backend on CPU).
+Deterministic mode (``deterministic=True``, ``set_deterministic(True)`` -- what ``Config.compute.deterministic`` does --
+or ``torch.use_deterministic_algorithms(True)``): the native backward computes dQ in a query-stationary kernel without
+atomics, so repeated backward passes give bitwise-equal gradients (cost: DESIGN.md section 7).
 Features the native kernels do not cover (dropout > 0, ALiBi, head_dim not in {64, 128}) route to ``sdpa`` /
 ``reference`` with a one-time warning rather than failing.
 """
@@ -27,6 +30,9 @@ from ..utils.logger import logger
 
 _BACKEND = os.environ.get("TORCHACC_B200_ATTN", "auto")
 _warned = set()
+_DETERMINISTIC = False
+# backward passes that ran the deterministic dQ kernel (tests check that the flag reached the kernels)
+DETERMINISTIC_BWD_CALLS = 0
 
 
 def set_attention_backend(name: str) -> None:
@@ -37,6 +43,17 @@ def set_attention_backend(name: str) -> None:
 
 def get_attention_backend() -> str:
     return _BACKEND
+
+
+def set_deterministic(flag: bool) -> None:
+    """Process-wide switch: every native attention backward takes the deterministic (atomic-free) dQ path."""
+    global _DETERMINISTIC
+    _DETERMINISTIC = bool(flag)
+
+
+def deterministic_enabled(flag: bool = False) -> bool:
+    """Effective flag: the per-call ``deterministic`` argument, the process switch or PyTorch's global switch."""
+    return bool(flag) or _DETERMINISTIC or torch.are_deterministic_algorithms_enabled()
 
 
 def _warn_once(key, msg):
@@ -56,6 +73,9 @@ nat.register_signatures({
     "tb_flash_attn_bwd_dropout": ([nat.u64] * 13 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
                                   [nat.i64] * 5 + [nat.i32, nat.u64, nat.i32, nat.u64, nat.i32, nat.f32, nat.u64],
                                   nat.i32),
+    "tb_flash_attn_bwd_deterministic": ([nat.u64] * 13 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
+                                        [nat.i64] * 5 + [nat.i32, nat.u64, nat.i32, nat.u64, nat.i32, nat.f32, nat.u64],
+                                        nat.i32),
 })
 
 
@@ -198,9 +218,25 @@ def _native_bwd(do3, q3, k3, v3, o3, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, 
     Tq, Hq, D = q3.shape
     ap, abs_ = _alibi_args(alibi, Hq)
     Tk, Hk = k3.shape[0], k3.shape[1]
-    dq_acc = torch.empty((Tq, Hq, D), dtype=torch.float32, device=q3.device)
     delta = torch.empty((Hq, Tq), dtype=torch.float32, device=q3.device)
     L = nat.require()
+    if deterministic:
+        # delta, dK/dV without the dQ step, then the query-stationary dQ kernel: no fp32 accumulator, no atomics
+        global DETERMINISTIC_BWD_CALLS
+        p, seed = dropout if dropout is not None else (0.0, 0)
+        nat.check(
+            L.tb_flash_attn_bwd_deterministic(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(),
+                                              do3.data_ptr(), lse.data_ptr(), dq3.data_ptr(), dk3.data_ptr(),
+                                              dv3.data_ptr(), 0, delta.data_ptr(), nat.ptr(cu_q), nat.ptr(cu_k), B,
+                                              Sq, Sk, Hq, Hk, D, q3.stride(0), k3.stride(0), v3.stride(0),
+                                              do3.stride(0), scale, int(causal), window[0], window[1], Tq, Tk,
+                                              dq3.stride(0), dk3.stride(0), dv3.stride(0), nat.num_sms(), nat.stream(),
+                                              int(q3.dtype == torch.bfloat16), ap, abs_, float(p), int(seed)),
+            "tb_flash_attn_bwd_deterministic")
+        nat.count_launch(3)
+        DETERMINISTIC_BWD_CALLS += 1
+        return
+    dq_acc = torch.empty((Tq, Hq, D), dtype=torch.float32, device=q3.device)
     if dropout is not None:
         nat.check(
             L.tb_flash_attn_bwd_dropout(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(), do3.data_ptr(),
@@ -245,8 +281,8 @@ class _FlashAttnFn(torch.autograd.Function):
         dq = torch.empty(q3.shape, dtype=q3.dtype, device=q3.device)
         dk = torch.empty(k3.shape, dtype=k3.dtype, device=k3.device)
         dv = torch.empty(v3.shape, dtype=v3.dtype, device=v3.device)
-        _native_bwd(do, q3, k3, v3, o, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, window, dq, dk, dv, det, ctx.alibi,
-                    ctx.dropout)
+        _native_bwd(do, q3, k3, v3, o, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, window, dq, dk, dv,
+                    deterministic_enabled(det), ctx.alibi, ctx.dropout)
         return dq, dk, dv, None, None, None, None, None, None, None, None, None, None, None
 
 
@@ -281,7 +317,8 @@ class _FlashAttnQKVPackedFn(torch.autograd.Function):
         dk3 = dqkv.as_strided((T, hk, d), (W, d, 1), hq * d)
         dv3 = dqkv.as_strided((T, hk, d), (W, d, 1), (hq + hk) * d)
         do3 = do.contiguous().view(T, hq, d)
-        _native_bwd(do3, q3, k3, v3, o, lse, cu, cu, B, S, S, scale, causal, window, dq3, dk3, dv3)
+        _native_bwd(do3, q3, k3, v3, o, lse, cu, cu, B, S, S, scale, causal, window, dq3, dk3, dv3,
+                    deterministic_enabled())
         return dqkv, None, None, None, None, None, None, None, None, None
 
 
@@ -374,7 +411,8 @@ def flash_attn_func(q, k, v, dropout_p=0.0, softmax_scale=None, causal=False, wi
 def flash_attn_qkvpacked_tokens(qkv, num_q_heads, num_kv_heads, head_dim, batch, seq_len, softmax_scale=None,
                                 causal=True, window_size=(-1, -1), cu_seqlens=None):
     """Native-model fast path.  qkv: [T, (Hq+2Hk)*D] (q|k|v along the last dim, T = batch*seq_len or packed with
-    ``cu_seqlens``).  Returns [T, Hq*D]."""
+    ``cu_seqlens``).  Returns [T, Hq*D].  The backward is deterministic when ``set_deterministic(True)`` or
+    ``torch.use_deterministic_algorithms(True)`` is in effect."""
     scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(head_dim)
     T = qkv.shape[0]
     hq, hk, d = num_q_heads, num_kv_heads, head_dim
@@ -397,7 +435,7 @@ def flash_attn_qkvpacked_tokens(qkv, num_q_heads, num_kv_heads, head_dim, batch,
 
 
 def flash_attn_varlen_cu(q3, k3, v3, cu_q, cu_k, scale, causal, window, return_lse=False, dropout_p=0.0,
-                         alibi_slopes=None):
+                         alibi_slopes=None, deterministic=False):
     """Packed sequences: q3 [Tq,Hq,D], k3/v3 [Tk,Hk,D], cu_* int32 [B+1]."""
     backend = _pick_backend(q3, k3, v3, dropout_p, alibi_slopes, pad_ok=True)
     Bn = cu_q.numel() - 1
@@ -405,8 +443,8 @@ def flash_attn_varlen_cu(q3, k3, v3, cu_q, cu_k, scale, causal, window, return_l
         (qp, kp, vp), D0 = _pad_head_dim(q3, k3, v3)
         alibi = alibi_slopes.float().contiguous() if alibi_slopes is not None else None
         dropout = (float(dropout_p), new_dropout_seed()) if dropout_p > 0.0 else None
-        o, lse = _FlashAttnFn.apply(qp, kp, vp, cu_q.int(), cu_k.int(), Bn, 0, 0, scale, causal, window, False, alibi,
-                                    dropout)
+        o, lse = _FlashAttnFn.apply(qp, kp, vp, cu_q.int(), cu_k.int(), Bn, 0, 0, scale, causal, window, deterministic,
+                                    alibi, dropout)
         o = o[..., :D0]
         return (o, lse) if return_lse else o
     assert dropout_p == 0.0 and alibi_slopes is None, "the per-sequence fallback handles plain attention only"
@@ -450,7 +488,7 @@ def flash_attn_varlen_func(q, k, v, attention_mask, dropout_p=0.0, softmax_scale
         o4, lse4 = attention_reference_masked(q, k, v, mask, scale, causal, window_size, alibi_slopes, dropout_p)
         return (o4, lse4, None) if return_attn_probs else o4
     res = flash_attn_varlen_cu(q3, k3, v3, cu, cu, scale, causal, tuple(window_size), return_lse=return_attn_probs,
-                               dropout_p=dropout_p, alibi_slopes=alibi_slopes)
+                               dropout_p=dropout_p, alibi_slopes=alibi_slopes, deterministic=deterministic)
     o3 = res[0] if return_attn_probs else res
     out = torch.zeros((B * Sq, Hq, D), dtype=q.dtype, device=q.device).index_copy(0, idx, o3).view(B, Sq, Hq, D)
     if return_attn_probs:
@@ -506,7 +544,7 @@ def flash_attn_varlen_position_ids_func(q, k, v, position_ids, dropout_p=0.0, so
     scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(D)
     cu = position_ids_to_cu_seqlens(position_ids)
     res = flash_attn_varlen_cu(q.reshape(S, Hq, D), k.reshape(S, Hk, D), v.reshape(S, Hk, D), cu, cu, scale, causal,
-                               tuple(window_size), return_lse=return_attn_probs)
+                               tuple(window_size), return_lse=return_attn_probs, deterministic=deterministic)
     if return_attn_probs:
         return res[0].view(1, S, Hq, D), res[1].view(Hq, 1, S).transpose(0, 1).contiguous(), None
     return res.view(1, S, Hq, D)

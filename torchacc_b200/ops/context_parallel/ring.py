@@ -461,6 +461,10 @@ def ring_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, q_lens: Op
         raise NotImplementedError("dropout is not supported by ring attention")
     if k_lens is not None and zigzag:
         raise NotImplementedError("variable-length K needs the contiguous (non-zigzag) layout")
+    if deterministic:
+        A._warn_once("ring-deterministic", "ring attention reduces dQ with atomics across its blocks: "
+                     "deterministic=True is not honoured by ring attention (its gradients may differ in the last bits "
+                     "from run to run)")
     scale = softmax_scale if softmax_scale is not None else 1.0 / math.sqrt(q.shape[-1])
     return _RingAttnFn.apply(q.contiguous(), k.contiguous(), v.contiguous(), scale, causal, tuple(window_size),
                              process_group, zigzag, impl, k_lens)

@@ -16,13 +16,47 @@ import torch
 
 from .. import _native as nat
 
+nat.register_signatures({
+    "tb_sqnorm_accumulate_ordered": ([nat.u64, nat.i32, nat.i64, nat.u64, nat.f32, nat.u64, nat.u64, nat.i32, nat.u64],
+                                     nat.i32),
+})
 
-def _sqnorm(t: torch.Tensor, out: torch.Tensor, pre_scale: float = 1.0):
+_DETERMINISTIC = False
+_ORDERED_WS = {}   # device -> (partials [8 * num_sms] fp32, ticket counter [1] int32)
+
+
+def set_deterministic(flag: bool) -> None:
+    """Process-wide switch: ``grad_sqnorm`` sums in a fixed order (bitwise reproducible gradient norms)."""
+    global _DETERMINISTIC
+    _DETERMINISTIC = bool(flag)
+
+
+def deterministic_enabled() -> bool:
+    """The process switch or PyTorch's ``torch.use_deterministic_algorithms``."""
+    return _DETERMINISTIC or torch.are_deterministic_algorithms_enabled()
+
+
+def _ordered_workspace(device: torch.device):
+    key = (device.type, device.index if device.index is not None else torch.cuda.current_device())
+    if key not in _ORDERED_WS:
+        _ORDERED_WS[key] = (torch.empty(8 * nat.num_sms(), dtype=torch.float32, device=device),
+                            torch.zeros(1, dtype=torch.int32, device=device))
+    return _ORDERED_WS[key]
+
+
+def _sqnorm(t: torch.Tensor, out: torch.Tensor, pre_scale: float = 1.0, ordered: bool = False):
     if nat.use_native(t) and t.dtype in (torch.bfloat16, torch.float32) and t.is_contiguous():
         L = nat.require()
-        nat.check(
-            L.tb_sqnorm_accumulate(t.data_ptr(), int(t.dtype == torch.bfloat16), t.numel(), out.data_ptr(),
-                                   pre_scale, nat.num_sms(), nat.stream()), "tb_sqnorm_accumulate")
+        if ordered:
+            partial, counter = _ordered_workspace(t.device)
+            nat.check(
+                L.tb_sqnorm_accumulate_ordered(t.data_ptr(), int(t.dtype == torch.bfloat16), t.numel(),
+                                               out.data_ptr(), pre_scale, partial.data_ptr(), counter.data_ptr(),
+                                               nat.num_sms(), nat.stream()), "tb_sqnorm_accumulate_ordered")
+        else:
+            nat.check(
+                L.tb_sqnorm_accumulate(t.data_ptr(), int(t.dtype == torch.bfloat16), t.numel(), out.data_ptr(),
+                                       pre_scale, nat.num_sms(), nat.stream()), "tb_sqnorm_accumulate")
         nat.count_launch()
     else:
         x = t.float() * pre_scale
@@ -32,12 +66,15 @@ def _sqnorm(t: torch.Tensor, out: torch.Tensor, pre_scale: float = 1.0):
 
 
 def grad_sqnorm(grads: Iterable[torch.Tensor], device=None) -> torch.Tensor:
-    """Returns a 2-element fp32 tensor ``[sum of squares, found_inf]`` accumulated over ``grads`` (no host sync)."""
+    """Returns a 2-element fp32 tensor ``[sum of squares, found_inf]`` accumulated over ``grads`` (no host sync).
+    In deterministic mode (``set_deterministic`` / ``torch.use_deterministic_algorithms``) the sums are taken in a
+    fixed order, so repeated calls on the same gradients are bitwise equal."""
     grads = [g for g in grads if g is not None]
     dev = device if device is not None else (grads[0].device if grads else torch.device("cpu"))
     out = torch.zeros(2, dtype=torch.float32, device=dev)
+    ordered = deterministic_enabled()
     for g in grads:
-        _sqnorm(g, out)
+        _sqnorm(g, out, ordered=ordered)
     return out
 
 

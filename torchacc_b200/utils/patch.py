@@ -52,18 +52,22 @@ def _hf_flash_attention_forward(query_states, key_states, value_states, attentio
                                 is_causal=True, dropout=0.0, position_ids=None, softmax_scale=None,
                                 sliding_window=None, use_top_left_mask=False, softcap=None, deterministic=None,
                                 **kwargs):
-    """Drop-in for ``transformers.modeling_flash_attention_utils._flash_attention_forward`` ([B,S,H,D] layout)."""
+    """Drop-in for ``transformers.modeling_flash_attention_utils._flash_attention_forward`` ([B,S,H,D] layout).
+    ``deterministic=None`` follows ``FLASH_ATTENTION_DETERMINISTIC=1``, as HF's own function does."""
     from ..ops import attention as A
     window = (sliding_window - 1, 0) if sliding_window else (-1, -1)
     causal = bool(is_causal) and not (use_top_left_mask and query_states.shape[1] == 1)
+    if deterministic is None:
+        deterministic = os.environ.get("FLASH_ATTENTION_DETERMINISTIC", "0") == "1"
     if attention_mask is not None and attention_mask.dim() == 2 and not bool(attention_mask.all()):
         return A.flash_attn_varlen_func(query_states, key_states, value_states, attention_mask, dropout, softmax_scale,
-                                        causal, window)
+                                        causal, window, deterministic=deterministic)
     if position_ids is not None and query_states.shape[0] == 1 and position_ids.numel() > 1 \
             and bool((position_ids.reshape(-1)[1:] == 0).any()):
         return A.flash_attn_varlen_position_ids_func(query_states, key_states, value_states, position_ids, dropout,
-                                                     softmax_scale, causal, window)
-    return A.flash_attn_func(query_states, key_states, value_states, dropout, softmax_scale, causal, window)
+                                                     softmax_scale, causal, window, deterministic=deterministic)
+    return A.flash_attn_func(query_states, key_states, value_states, dropout, softmax_scale, causal, window,
+                             deterministic=deterministic)
 
 
 def patch_fa() -> bool:
