@@ -310,6 +310,66 @@ TB_API int tb_gemm_mxfp8(uint64_t A, uint64_t sfa, uint64_t B, uint64_t sfb, uin
   return (int)tb::gemm_mxfp8(P<void>(A), P<void>(sfa), P<void>(B), P<void>(sfb), P<void>(D), P<void>(C), M, N, K, lda, ldb,
                              ldd, ldc, out_fp32 != 0, num_sms, S(stream));
 }
+// ---- mixture of experts: grouped GEMMs (gemm/gemm_bf16.cu) and routing kernels (ops/moe.cu) --------------------
+TB_API int tb_gemm_grouped(uint64_t A, uint64_t B, uint64_t D, int M, int N, int K, int E, long long lda, long long ldb,
+                           long long ldd, int b_mn_major, uint64_t tile_expert, uint64_t num_m_tiles, int num_sms,
+                           uint64_t stream, int is_fp16) {
+  return (int)tb::gemm_grouped_bf16(P<void>(A), P<void>(B), P<void>(D), M, N, K, E, lda, ldb, ldd, b_mn_major != 0,
+                                    P<const int>(tile_expert), P<const int>(num_m_tiles), num_sms, S(stream),
+                                    is_fp16 != 0);
+}
+TB_API int tb_gemm_grouped_swiglu(uint64_t A, uint64_t Wgu, uint64_t H, uint64_t GU, int M, int F, int K, int E,
+                                  long long lda, long long ldb, long long ldh, long long ldgu, uint64_t tile_expert,
+                                  uint64_t num_m_tiles, int num_sms, uint64_t stream, int is_fp16) {
+  return (int)tb::gemm_grouped_swiglu_bf16(P<void>(A), P<void>(Wgu), P<void>(H), P<void>(GU), M, F, K, E, lda, ldb, ldh,
+                                           ldgu, P<const int>(tile_expert), P<const int>(num_m_tiles), num_sms,
+                                           S(stream), is_fp16 != 0);
+}
+TB_API int tb_gemm_grouped_wgrad(uint64_t dY, uint64_t X, uint64_t D, int M, int N, int E, int rows, long long lda,
+                                 long long ldb, long long ldd, uint64_t offsets, int out_fp32, int accumulate,
+                                 int num_sms, uint64_t stream, int is_fp16) {
+  return (int)tb::gemm_grouped_wgrad_bf16(P<void>(dY), P<void>(X), P<void>(D), M, N, E, rows, lda, ldb, ldd,
+                                          P<const int>(offsets), out_fp32 != 0, accumulate != 0, num_sms, S(stream),
+                                          is_fp16 != 0);
+}
+// router logits dtype: 0 = fp32, 1 = bf16, 2 = fp16
+TB_API int tb_moe_router_fwd(uint64_t logits, uint64_t weights, uint64_t ids, int T, int E, int k, int norm_topk,
+                             int dtype, uint64_t stream) {
+  return (int)tb::moe_router_fwd(P<void>(logits), P<float>(weights), P<long long>(ids), T, E, k, norm_topk != 0, dtype,
+                                 S(stream));
+}
+TB_API int tb_moe_router_bwd(uint64_t logits, uint64_t ids, uint64_t dweights, uint64_t dlogits, int T, int E, int k,
+                             int norm_topk, int dtype, uint64_t stream) {
+  return (int)tb::moe_router_bwd(P<void>(logits), P<long long>(ids), P<float>(dweights), P<void>(dlogits), T, E, k,
+                                 norm_topk != 0, dtype, S(stream));
+}
+TB_API int tb_moe_index(uint64_t ids, int T, int k, int E, int rows, uint64_t counts, uint64_t offsets,
+                        uint64_t tile_expert, uint64_t num_m_tiles, uint64_t pos, uint64_t row_src, uint64_t stream) {
+  return (int)tb::moe_index(P<long long>(ids), T, k, E, rows, P<int>(counts), P<int>(offsets), P<int>(tile_expert),
+                            P<int>(num_m_tiles), P<int>(pos), P<int>(row_src), S(stream));
+}
+TB_API int tb_moe_permute(uint64_t x, uint64_t row_src, uint64_t offsets, uint64_t x_perm, int rows, int k, int E, int H,
+                          int num_sms, uint64_t stream) {
+  return (int)tb::moe_permute(P<void>(x), P<int>(row_src), P<int>(offsets), P<void>(x_perm), rows, k, E, H, num_sms,
+                              S(stream));
+}
+TB_API int tb_moe_unpermute_sum(uint64_t dx_perm, uint64_t pos, uint64_t dx, int T, int k, int H, int num_sms,
+                                uint64_t stream, int is_bf16) {
+  return (int)tb::moe_unpermute_sum(P<void>(dx_perm), P<int>(pos), P<void>(dx), T, k, H, num_sms, is_bf16 != 0,
+                                    S(stream));
+}
+TB_API int tb_moe_combine_fwd(uint64_t y_perm, uint64_t pos, uint64_t w, uint64_t residual, uint64_t out, int T, int k,
+                              int H, int num_sms, uint64_t stream, int is_bf16) {
+  return (int)tb::moe_combine_fwd(P<void>(y_perm), P<int>(pos), P<float>(w), P<void>(residual), P<void>(out), T, k, H,
+                                  num_sms, is_bf16 != 0, S(stream));
+}
+TB_API int tb_moe_combine_bwd(uint64_t dout, uint64_t y_perm, uint64_t row_src, uint64_t offsets, uint64_t w,
+                              uint64_t dy_perm, uint64_t dw, int rows, int k, int E, int H, int num_sms,
+                              uint64_t stream, int is_bf16) {
+  return (int)tb::moe_combine_bwd(P<void>(dout), P<void>(y_perm), P<int>(row_src), P<int>(offsets), P<float>(w),
+                                  P<void>(dy_perm), P<float>(dw), rows, k, E, H, num_sms, is_bf16 != 0, S(stream));
+}
+
 TB_API int tb_gemm_swiglu(uint64_t A, uint64_t Wgu, uint64_t H, uint64_t GU, int M, int F, int K, long long lda,
                           long long ldb, long long ldh, long long ldgu, int num_sms, uint64_t stream, int is_fp16) {
   return (int)tb::gemm_swiglu_bf16(P<void>(A), P<void>(Wgu), P<void>(H), P<void>(GU), M, F, K, lda, ldb, ldh, ldgu, num_sms,

@@ -32,6 +32,26 @@ cudaError_t gemm_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, 
                              long long ldb, long long ldh, long long ldgu, int num_sms, cudaStream_t stream,
                              bool is_fp16 = false);
 
+// ---- grouped (mixture-of-experts) GEMMs over expert-sorted rows (see GroupArgs in gemm_bf16.cu) ----
+// Rows of A are tokens sorted by expert, every expert's segment padded with zero rows to a multiple of 128; M is the
+// padded row capacity (a multiple of 128).  tile_expert[m_tile] is the expert of each 128-row tile and *num_m_tiles
+// the number of valid tiles; both stay on the device.
+// D[M, N] = A[M, K] B_e^T: B is [E*N][K] (b_mn_major == false, forward) or [E*K][N] (true, dgrad: B_e read transposed).
+cudaError_t gemm_grouped_bf16(const void* A, const void* B, void* D, int M, int N, int K, int E, long long lda,
+                              long long ldb, long long ldd, bool b_mn_major, const int* tile_expert,
+                              const int* num_m_tiles, int num_sms, cudaStream_t stream, bool is_fp16 = false);
+// gate|up projection with the SwiGLU epilogue per expert: W_gu is [E*2F][K], expert e's gate rows start at e*2F and its
+// up rows at e*2F + F.  F % 128 == 0.
+cudaError_t gemm_grouped_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, int M, int F, int K, int E,
+                                     long long lda, long long ldb, long long ldh, long long ldgu,
+                                     const int* tile_expert, const int* num_m_tiles, int num_sms, cudaStream_t stream,
+                                     bool is_fp16 = false);
+// wgrad: D[e*M : e*M + M, N] (+)= dY_e^T X_e, reducing over expert e's padded rows [offsets[e], offsets[e+1]) of
+// dY [rows][M] and X [rows][N].  An expert without rows writes zeros (or leaves D unchanged when accumulating).
+cudaError_t gemm_grouped_wgrad_bf16(const void* dY, const void* X, void* D, int M, int N, int E, int rows,
+                                    long long lda, long long ldb, long long ldd, const int* offsets, bool out_fp32,
+                                    bool accumulate, int num_sms, cudaStream_t stream, bool is_fp16 = false);
+
 // ---- fused tensor-parallel kernels (see the FuseArgs comment in gemm_bf16.cu) ----
 // all-gather -> GEMM: D[world*rows, N] = gather(A)[world*rows, K] * B_op^T.  `a_full` is this rank's symmetric
 // gathered buffer whose own row block is already filled; `peer_a_full[r]` is rank r's mapping of the same buffer.

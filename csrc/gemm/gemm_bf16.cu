@@ -63,6 +63,24 @@ struct FuseArgs {
   long long slot_stride;          // kFuse 2: elements between two source slots of a staging buffer
 };
 
+// Grouped (mixture-of-experts) mode, a compile-time switch of the kernel (kGroup; 0 = the dense GEMM).  The A rows
+// are tokens sorted by expert, each expert's segment padded with zero rows to a multiple of kBlockM, so that no
+// 128-row tile and no 64-row K block straddles two experts.  Expert weights are one flat 2-D tensor.
+//   kGroup == 1 (forward, dgrad, SwiGLU gate|up):  D[Mp, N] = A[Mp, K] B_e^T with e = tile_expert[m_tile].
+//     B is [E * b_rows, K] (K-major: expert e starts at row e * b_rows) or [E * b_rows, N] (MN-major: the K coordinate
+//     moves by e * b_rows).  The grid covers the upper bound of row tiles; the real count lives on the device and
+//     tiles past it exit at once.
+//   kGroup == 2 (wgrad):  D_e[M, N] = A_e^T B_e for every expert, A = dY [Mp, M] and B = X [Mp, N] both MN-major,
+//     the reduction running over the expert's padded row range [offsets[e], offsets[e+1]).  D is [E * M, N].
+//     An expert without rows writes zeros (or leaves D unchanged when accumulating).
+struct GroupArgs {
+  const int* tile_expert;  // kGroup 1
+  const int* num_m_tiles;  // kGroup 1: device-resident count of valid row tiles
+  const int* offsets;      // kGroup 2: [E + 1] padded row offsets
+  int num_experts;         // kGroup 2
+  int b_rows;              // kGroup 1: rows of one expert in the flat B
+};
+
 struct GemmArgs {
   void* D;
   const __nv_bfloat16* bias;
@@ -82,6 +100,7 @@ struct GemmArgs {
   int dynamic;     // 1: grid = one CTA per tile instead of a persistent grid (see gemm_sched_mode)
   FuseArgs fuse;
   CarryArgs carry;  // slices of pending FSDP collectives moved by warp 3 of every CTA while the tiles run (fused/carry.cuh)
+  GroupArgs group;
 };
 
 TB_DEVICE void st_release_sys_u32(uint32_t* p, uint32_t v) {
@@ -221,13 +240,15 @@ __device__ __forceinline__ void tile_coords_sharded(int t, int tiles_m_per_shard
   tn = ln;
 }
 
-template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmArgs args) {
   using S = GemmSmem;
   constexpr int kStages = S::kStages;
   constexpr int kTA = (kAMajor == Major::MN) ? 1 : 0, kTB = (kBMajor == Major::MN) ? 1 : 0;
+  static_assert(kGroup == 0 || kFuse == 0, "grouped GEMMs are not fused with collectives");
+  static_assert(kGroup != 2 || (kAMajor == Major::MN && kBMajor == Major::MN), "grouped wgrad reads both operands MN-major");
 
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024-byte alignment.
@@ -241,8 +262,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const uint32_t lane = lane_id();
 
-  const int num_tiles = args.num_m_tiles * args.num_n_tiles;
+  int num_m_tiles = args.num_m_tiles;
+  if constexpr (kGroup == 1) num_m_tiles = *args.group.num_m_tiles;
+  const int tiles_per_expert = num_m_tiles * args.num_n_tiles;
+  const int num_tiles = (kGroup == 2) ? args.group.num_experts * tiles_per_expert : tiles_per_expert;
   const int num_k_blocks = (args.K + kBlockK - 1) / kBlockK;
+  // grouped wgrad: the K loop covers the padded rows of expert e (multiples of kBlockM, so whole K blocks)
+  auto expert_k_blocks = [&](int e, int& k_base) {
+    k_base = args.group.offsets[e];
+    return (args.group.offsets[e + 1] - k_base) / kBlockK;
+  };
   int cta = blockIdx.x;
   int num_ctas = gridDim.x;
   if constexpr (kFuse == 1) {
@@ -257,12 +286,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   const int tiles_m_per_shard = (kFuse != 0) ? args.fuse.rows_per_rank / kBlockM : 0;
   // fused tile order: all-gather starts with the local row block; reduce-scatter ends with it (peers first)
   const int first_shard = (kFuse == 1) ? args.fuse.rank : ((kFuse == 2) ? (args.fuse.rank + 1) % args.fuse.world : 0);
+  // `shard`: the row block of the fused variants, the expert of the grouped wgrad, 0 otherwise
   auto coords = [&](int t, int& tm, int& tn, int& shard) {
     if constexpr (kFuse != 0) {
       tile_coords_sharded(t, tiles_m_per_shard, args.num_n_tiles, first_shard, args.fuse.world, tm, tn, shard);
+    } else if constexpr (kGroup == 2) {
+      shard = t / tiles_per_expert;
+      tile_coords(t - shard * tiles_per_expert, num_m_tiles, args.num_n_tiles, tm, tn);
     } else {
       shard = 0;
-      tile_coords(t, args.num_m_tiles, args.num_n_tiles, tm, tn);
+      tile_coords(t, num_m_tiles, args.num_n_tiles, tm, tn);
     }
   };
 
@@ -300,11 +333,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
               fence_proxy_async_all();       // generic-proxy writes of the copy CTAs -> visible to TMA
             }
           }
-          for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
+          int nkb = num_k_blocks, k_base = 0, b_off = 0;   // b_off: the expert's offset in the flat B
+          if constexpr (kGroup == 1) b_off = args.group.tile_expert[tm] * args.group.b_rows;
+          if constexpr (kGroup == 2) nkb = expert_k_blocks(shard, k_base);
+          for (int kb = 0; kb < nkb; ++kb, ++it) {
             const int s = it % kStages;
             mbar_wait(empty_bar(s), ((it / kStages) & 1) ^ 1);
             mbar_arrive_expect_tx(full_bar(s), S::kStageBytes);
-            const int k0 = kb * kBlockK;
+            const int k0 = k_base + kb * kBlockK;
             if constexpr (kAMajor == Major::K) {
               tma_load_2d(smem_a(s), &tmap_a, full_bar(s), k0, m0);
             } else {
@@ -313,12 +349,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                 tma_load_2d(smem_a(s) + i * 8192, &tmap_a, full_bar(s), m0 + i * 64, k0);
             }
             if constexpr (kBMajor == Major::K) {
-              tma_load_2d(smem_b(s), &tmap_b, full_bar(s), k0, n0);
-              tma_load_2d(smem_b(s) + S::kBBytes / 2, &tmap_b, full_bar(s), k0, n1);
+              tma_load_2d(smem_b(s), &tmap_b, full_bar(s), k0, b_off + n0);
+              tma_load_2d(smem_b(s) + S::kBBytes / 2, &tmap_b, full_bar(s), k0, b_off + n1);
             } else {
 #pragma unroll
               for (int i = 0; i < kBlockN / 64; ++i)
-                tma_load_2d(smem_b(s) + i * 8192, &tmap_b, full_bar(s), n0 + i * 64, k0);
+                tma_load_2d(smem_b(s) + i * 8192, &tmap_b, full_bar(s), n0 + i * 64, b_off + k0);
             }
           }
         }
@@ -369,8 +405,25 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     for (int t = cta; t < num_tiles; t += num_ctas) {
       int tm, tn, shard;
       coords(t, tm, tn, shard);
+      int nkb = num_k_blocks, k_base;
+      if constexpr (kGroup == 2) {
+        nkb = expert_k_blocks(shard, k_base);
+        if (nkb == 0) {   // expert without rows: its gradient is zero; when accumulating, D stays as it is
+          if (args.C == nullptr) {
+            const int col = tn * kBlockN + (int)(threadIdx.x - 128);
+            for (int r = 0; r < kBlockM && col < args.N; ++r) {
+              const long long row = (long long)tm * kBlockM + r;
+              if (row >= args.M) break;
+              const long long off = ((long long)shard * args.M + row) * args.ldd + col;
+              if (args.out_fp32) reinterpret_cast<float*>(args.D)[off] = 0.f;
+              else reinterpret_cast<uint16_t*>(args.D)[off] = 0;
+            }
+          }
+          continue;
+        }
+      }
       float acc[kBlockN / 2];
-      for (int kb = 0; kb < num_k_blocks; ++kb, ++it) {
+      for (int kb = 0; kb < nkb; ++kb, ++it) {
         const int s = it % kStages;
         mbar_wait(full_bar(s), (it / kStages) & 1);
         wgmma_fence_acc(acc);
@@ -464,6 +517,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
       const int n0 = tn * kBlockN;
       const uint16_t* bias = reinterpret_cast<const uint16_t*>(args.bias);
+      // grouped wgrad: expert `shard` owns rows [shard * M, shard * M + M) of D (and of C); 0 for every other mode
+      const long long erow = (kGroup == 2) ? (long long)shard * args.M : 0;
       if (args.out_fp32) {
         // fp32 output: the four lanes of a quad already cover 32 contiguous bytes of a row
         const bool vec = (args.ldd % 2 == 0) && (args.C == nullptr || args.ldc % 2 == 0) &&
@@ -479,8 +534,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             const long long grow = row0 + 8 * half;
             if (grow >= args.M) continue;
             float v0 = acc[4 * j + 2 * half] + b0, v1 = acc[4 * j + 2 * half + 1] + b1;
-            float* dp = reinterpret_cast<float*>(args.D) + grow * args.ldd + col;
-            const float* cp = args.C ? reinterpret_cast<const float*>(args.C) + grow * args.ldc + col : nullptr;
+            float* dp = reinterpret_cast<float*>(args.D) + (erow + grow) * args.ldd + col;
+            const float* cp = args.C ? reinterpret_cast<const float*>(args.C) + (erow + grow) * args.ldc + col : nullptr;
             if (two && vec) {
               if (cp) {
                 const float2 old = *reinterpret_cast<const float2*>(cp);
@@ -517,7 +572,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
                   if (two) v1 += ld1(bias + col + 1);
                 }
                 if (args.C) {
-                  const uint16_t* cp = reinterpret_cast<const uint16_t*>(args.C) + grow * args.ldc + col;
+                  const uint16_t* cp = reinterpret_cast<const uint16_t*>(args.C) + (erow + grow) * args.ldc + col;
                   if (two && pair_c) {
                     const float2 old = unpack_h2<kBf16>(*reinterpret_cast<const uint32_t*>(cp));
                     v0 += old.x; v1 += old.y;
@@ -532,7 +587,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
             quad_transpose(x, lane);
             const int col = n0 + 32 * g + 8 * (int)quad;
             if (row_ok && col < args.N)
-              store_row8(reinterpret_cast<uint16_t*>(args.D) + grow * args.ldd + col, x, args.N - col, vec_d);
+              store_row8(reinterpret_cast<uint16_t*>(args.D) + (erow + grow) * args.ldd + col, x, args.N - col, vec_d);
           }
         }
       }
@@ -547,11 +602,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // ------------------------------------------------------------------------------------------------------
 // Host launcher
 // ------------------------------------------------------------------------------------------------------
-template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, const GemmArgs& args, int num_sms,
                               cudaStream_t stream) {
   using S = GemmSmem;
-  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse>;
+  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse, kGroup>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotalCarry);
@@ -559,7 +614,8 @@ static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, con
     configured = true;
   }
   const bool carrying = kFuse == 0 && args.carry.slice[0].kind != 0;
-  const int num_tiles = args.num_m_tiles * args.num_n_tiles;
+  // grouped forward: the upper bound of row tiles (the real count is only known on the device)
+  const int num_tiles = args.num_m_tiles * args.num_n_tiles * (kGroup == 2 ? args.group.num_experts : 1);
   const int comm_ctas = (kFuse == 1) ? args.fuse.comm_clusters * kCommCtasPerCluster : 0;
   int ctas = num_sms - comm_ctas;   // copy CTAs share their SMs with nobody
   if (ctas > num_tiles) ctas = num_tiles;
@@ -597,6 +653,7 @@ static bool fill_common(GemmArgs& args, void* D, const void* bias, int M, int N,
   args.swiglu = 0; args.swiglu_F = 0; args.gu_out = nullptr; args.ldgu = 0;
   memset(&args.fuse, 0, sizeof(args.fuse));
   memset(&args.carry, 0, sizeof(args.carry));
+  memset(&args.group, 0, sizeof(args.group));
   return true;
 }
 
@@ -669,6 +726,89 @@ cudaError_t gemm_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, 
   carry_take(4.0 * (double)M * (double)F * (double)K, &args.carry);
   if (is_fp16) return launch_one<false, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
   return launch_one<true, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
+}
+
+// ------------------------------------------------------------------------------------------------------
+// Grouped (mixture-of-experts) entry points (see the GroupArgs comment).  No carried collectives ride along.
+// ------------------------------------------------------------------------------------------------------
+cudaError_t gemm_grouped_bf16(const void* A, const void* B, void* D, int M, int N, int K, int E, long long lda,
+                              long long ldb, long long ldd, bool b_mn_major, const int* tile_expert,
+                              const int* num_m_tiles, int num_sms, cudaStream_t stream, bool is_fp16) {
+  if (M <= 0 || N <= 0) return cudaSuccess;
+  if (K <= 0 || E <= 0 || M % kBlockM != 0 || tile_expert == nullptr || num_m_tiles == nullptr)
+    return cudaErrorInvalidValue;
+  CUtensorMap ta, tbm;
+  try {
+    ta = operand_map(A, M, K, lda, false, kBlockM);
+    tbm = b_mn_major ? operand_map(B, N, E * K, ldb, true, kBlockN / 2)
+                     : operand_map(B, E * N, K, ldb, false, kBlockN / 2);
+  } catch (const std::exception& e) {
+    fprintf(stderr, "%s\n", e.what());
+    return cudaErrorInvalidValue;
+  }
+  GemmArgs args;
+  fill_common(args, D, nullptr, M, N, K, ldd, false, nullptr, 0);
+  args.dynamic = 0;
+  args.group.tile_expert = tile_expert;
+  args.group.num_m_tiles = num_m_tiles;
+  args.group.b_rows = b_mn_major ? K : N;
+  if (is_fp16) {
+    if (b_mn_major) return launch_one<false, Major::K, Major::MN, 0, 1>(ta, tbm, args, num_sms, stream);
+    return launch_one<false, Major::K, Major::K, 0, 1>(ta, tbm, args, num_sms, stream);
+  }
+  if (b_mn_major) return launch_one<true, Major::K, Major::MN, 0, 1>(ta, tbm, args, num_sms, stream);
+  return launch_one<true, Major::K, Major::K, 0, 1>(ta, tbm, args, num_sms, stream);
+}
+
+cudaError_t gemm_grouped_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, int M, int F, int K, int E,
+                                     long long lda, long long ldb, long long ldh, long long ldgu,
+                                     const int* tile_expert, const int* num_m_tiles, int num_sms, cudaStream_t stream,
+                                     bool is_fp16) {
+  if (M <= 0 || F <= 0) return cudaSuccess;
+  if (K <= 0 || E <= 0 || M % kBlockM != 0 || F % 128 != 0 || ldh % 8 != 0 || (GU != nullptr && ldgu % 8 != 0))
+    return cudaErrorInvalidValue;
+  if (reinterpret_cast<uintptr_t>(H) % 16 != 0 || reinterpret_cast<uintptr_t>(GU) % 16 != 0) return cudaErrorInvalidValue;
+  if (tile_expert == nullptr || num_m_tiles == nullptr) return cudaErrorInvalidValue;
+  CUtensorMap ta, tbm;
+  try {
+    ta = make_map_2d_bf16(A, M, K, lda, kBlockK, kBlockM);
+    tbm = make_map_2d_bf16(Wgu, 2 * (uint64_t)F * E, K, ldb, kBlockK, kBlockN / 2);
+  } catch (const std::exception& e) {
+    fprintf(stderr, "%s\n", e.what());
+    return cudaErrorInvalidValue;
+  }
+  GemmArgs args;
+  fill_common(args, H, nullptr, M, F, K, ldh, false, nullptr, 0);
+  args.num_n_tiles = F / 128;
+  args.swiglu = 1; args.swiglu_F = F; args.gu_out = GU; args.ldgu = ldgu;
+  args.dynamic = 0;
+  args.group.tile_expert = tile_expert;
+  args.group.num_m_tiles = num_m_tiles;
+  args.group.b_rows = 2 * F;
+  if (is_fp16) return launch_one<false, Major::K, Major::K, 0, 1>(ta, tbm, args, num_sms, stream);
+  return launch_one<true, Major::K, Major::K, 0, 1>(ta, tbm, args, num_sms, stream);
+}
+
+cudaError_t gemm_grouped_wgrad_bf16(const void* dY, const void* X, void* D, int M, int N, int E, int rows,
+                                    long long lda, long long ldb, long long ldd, const int* offsets, bool out_fp32,
+                                    bool accumulate, int num_sms, cudaStream_t stream, bool is_fp16) {
+  if (M <= 0 || N <= 0 || E <= 0) return cudaSuccess;
+  if (rows <= 0 || rows % kBlockM != 0 || offsets == nullptr) return cudaErrorInvalidValue;
+  CUtensorMap ta, tbm;
+  try {
+    ta = operand_map(dY, M, rows, lda, true, kBlockM);
+    tbm = operand_map(X, N, rows, ldb, true, kBlockN / 2);
+  } catch (const std::exception& e) {
+    fprintf(stderr, "%s\n", e.what());
+    return cudaErrorInvalidValue;
+  }
+  GemmArgs args;
+  fill_common(args, D, nullptr, M, N, rows, ldd, out_fp32, accumulate ? D : nullptr, ldd);
+  args.dynamic = 0;
+  args.group.offsets = offsets;
+  args.group.num_experts = E;
+  if (is_fp16) return launch_one<false, Major::MN, Major::MN, 0, 2>(ta, tbm, args, num_sms, stream);
+  return launch_one<true, Major::MN, Major::MN, 0, 2>(ta, tbm, args, num_sms, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------

@@ -34,6 +34,27 @@ cudaError_t sqnorm_accumulate_ordered(const void* g, bool is_bf16, long long n, 
 // matrix x[R][C]; either pair may be null.
 cudaError_t quant_mxfp8(const void* x, long long ldx, int R, int C, void* q, long long ldq, void* sf, void* qt,
                         long long ldqt, void* sft, cudaStream_t stream);
+// Mixture-of-experts routing (ops/moe.cu), deterministic: see the comment at the top of that file.
+// Router: softmax over E <= 256 logits (dtype 0 = fp32, 1 = bf16, 2 = fp16), top-k <= 8, optional renormalisation of
+// the k fp32 weights; the backward maps d(weights) to d(logits).
+cudaError_t moe_router_fwd(const void* logits, float* weights, long long* ids, int T, int E, int k, bool norm,
+                           int dtype, cudaStream_t stream);
+cudaError_t moe_router_bwd(const void* logits, const long long* ids, const float* dweights, void* dlogits, int T, int E,
+                           int k, bool norm, int dtype, cudaStream_t stream);
+// Index build for ids [T*k]: counts [E], 128-row padded offsets [E+1], tile_expert [rows/128], *num_m_tiles, pos [T*k]
+// (row of each entry, stable order inside an expert) and row_src [rows] (entry of each row, -1 for padding).
+// rows >= T*k + E*127, rows % 128 == 0.
+cudaError_t moe_index(const long long* ids, int T, int k, int E, int rows, int* counts, int* offsets, int* tile_expert,
+                      int* num_m_tiles, int* pos, int* row_src, cudaStream_t stream);
+cudaError_t moe_permute(const void* x, const int* row_src, const int* offsets, void* x_perm, int rows, int k, int E,
+                        int H, int num_sms, cudaStream_t stream);
+cudaError_t moe_unpermute_sum(const void* dx_perm, const int* pos, void* dx, int T, int k, int H, int num_sms,
+                              bool is_bf16, cudaStream_t stream);
+cudaError_t moe_combine_fwd(const void* y_perm, const int* pos, const float* w, const void* residual, void* out, int T,
+                            int k, int H, int num_sms, bool is_bf16, cudaStream_t stream);
+cudaError_t moe_combine_bwd(const void* dout, const void* y_perm, const int* row_src, const int* offsets, const float* w,
+                            void* dy_perm, float* dw, int rows, int k, int E, int H, int num_sms, bool is_bf16,
+                            cudaStream_t stream);
 cudaError_t scale_inplace(void* g, bool is_bf16, long long n, const float* scale, int num_sms, cudaStream_t stream);
 
 }  // namespace tb

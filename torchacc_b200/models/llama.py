@@ -25,6 +25,7 @@ from ..ops.cross_entropy import fused_linear_cross_entropy
 from ..ops.linear import linear
 from ..ops.rmsnorm import rmsnorm
 from ..ops.rope import rope_qkv_, rope_tables
+from ..ops.moe import MoEMLP, load_balancing_loss
 from ..ops.swiglu import gate_up_swiglu, swiglu
 
 
@@ -47,26 +48,43 @@ class LlamaConfig:
     initializer_range: float = 0.02
     loss_chunk_tokens: int = 4096
     model_type: str = "llama"
+    # mixture of experts (Mixtral style): 0 = dense MLP.  Each token runs num_experts_per_tok experts of width
+    # moe_intermediate_size (default: intermediate_size), chosen by a softmax -> top-k router.
+    num_experts: int = 0
+    num_experts_per_tok: int = 2
+    moe_intermediate_size: Optional[int] = None
+    norm_topk_prob: bool = True
+    router_aux_loss_coef: float = 0.0     # load-balancing loss weight, same scale as HF Mixtral's (0.02 there)
 
     def __post_init__(self):
         if self.head_dim is None:
             self.head_dim = self.hidden_size // self.num_attention_heads
+        if self.num_experts and self.moe_intermediate_size is None:
+            self.moe_intermediate_size = self.intermediate_size
+
+    def _mlp_params(self) -> int:
+        """MLP parameters one token uses (for MoE: the router and the k active experts)."""
+        h = self.hidden_size
+        if self.num_experts:
+            return h * self.num_experts + self.num_experts_per_tok * 3 * h * self.moe_intermediate_size
+        return 3 * h * self.intermediate_size
 
     @property
     def qkv_dim(self):
         return (self.num_attention_heads + 2 * self.num_key_value_heads) * self.head_dim
 
     def num_params(self) -> int:
-        h, f, v, L = self.hidden_size, self.intermediate_size, self.vocab_size, self.num_hidden_layers
-        per = self.qkv_dim * h + h * self.num_attention_heads * self.head_dim + 3 * h * f + 2 * h
+        """Active parameters per token (all parameters for a dense model)."""
+        h, v, L = self.hidden_size, self.vocab_size, self.num_hidden_layers
+        per = self.qkv_dim * h + h * self.num_attention_heads * self.head_dim + self._mlp_params() + 2 * h
         if self.attention_bias:
             per += self.qkv_dim
         return L * per + v * h * (1 if self.tie_word_embeddings else 2) + h
 
     def flops_per_token(self, seq_len: int, causal: bool = True) -> float:
         """Training FLOPs per token (fwd + bwd = 3x fwd), GEMMs + attention."""
-        h, f, L = self.hidden_size, self.intermediate_size, self.num_hidden_layers
-        gemm = 2 * (self.qkv_dim * h + h * self.num_attention_heads * self.head_dim + 3 * h * f) * L
+        h, L = self.hidden_size, self.num_hidden_layers
+        gemm = 2 * (self.qkv_dim * h + h * self.num_attention_heads * self.head_dim + self._mlp_params()) * L
         gemm += 2 * self.vocab_size * h
         attn = 4 * seq_len * self.num_attention_heads * self.head_dim * L * (0.5 if causal else 1.0)
         return 3.0 * (gemm + attn)
@@ -91,6 +109,11 @@ PRESETS = {
                          max_position_embeddings=32768),
     "tiny": dict(vocab_size=512, hidden_size=256, intermediate_size=512, num_hidden_layers=2, num_attention_heads=4,
                  num_key_value_heads=2, head_dim=64, max_position_embeddings=512),
+    "mixtral-8x7b": dict(vocab_size=32000, intermediate_size=14336, num_key_value_heads=8, rope_theta=1000000.0,
+                         max_position_embeddings=32768, num_experts=8, num_experts_per_tok=2, model_type="mixtral"),
+    "tiny-moe": dict(vocab_size=512, hidden_size=256, intermediate_size=256, num_hidden_layers=2, num_attention_heads=4,
+                     num_key_value_heads=2, head_dim=64, max_position_embeddings=512, num_experts=8,
+                     num_experts_per_tok=2, model_type="mixtral"),
 }
 
 
@@ -182,7 +205,11 @@ class LlamaDecoderLayer(nn.Module):
         self.input_layernorm = _NormWeight(cfg.hidden_size, cfg.rms_norm_eps, **kw)
         self.self_attn = LlamaAttention(cfg, layer_idx, **kw)
         self.post_attention_layernorm = _NormWeight(cfg.hidden_size, cfg.rms_norm_eps, **kw)
-        self.mlp = LlamaMLP(cfg, **kw)
+        if cfg.num_experts:
+            self.mlp = MoEMLP(cfg.hidden_size, cfg.moe_intermediate_size, cfg.num_experts, cfg.num_experts_per_tok,
+                              cfg.norm_topk_prob, **kw)
+        else:
+            self.mlp = LlamaMLP(cfg, **kw)
 
     def forward(self, h, rope, batch, seq_len, position_ids=None, cu_seqlens=None, pctx=None):
         w1, w2 = self.input_layernorm.weight, self.post_attention_layernorm.weight
@@ -195,6 +222,8 @@ class LlamaDecoderLayer(nn.Module):
         y, h_skip = rmsnorm(h, w1, self.input_layernorm.eps, passthrough=True)
         a = self.self_attn(y, rope, batch, seq_len, position_ids, cu_seqlens, pctx)
         y2, h2 = rmsnorm(a, w2, self.post_attention_layernorm.eps, residual=h_skip)
+        if isinstance(self.mlp, MoEMLP):
+            return self.mlp(y2, residual=h2)          # residual added in the combine kernel
         return self.mlp(y2, pctx, residual=h2)
 
 
@@ -326,6 +355,9 @@ class LlamaForCausalLM(nn.Module):
                 out["loss"] = fused_linear_cross_entropy(hidden, self.lm_head.weight, lab.reshape(-1),
                                                          chunk_tokens=self.config.loss_chunk_tokens,
                                                          n_valid_total=n_valid_total)
+            if self.config.num_experts and self.config.router_aux_loss_coef:
+                out["aux_loss"] = self.router_aux_loss()
+                out["loss"] = out["loss"] + self.config.router_aux_loss_coef * out["aux_loss"]
         if return_logits or (labels is None and return_logits is None):
             tp = self.model.pctx.tp
             if self.model.pctx.cp_mesh is not None:
@@ -341,10 +373,17 @@ class LlamaForCausalLM(nn.Module):
                 out["logits"] = linear(hidden, self.lm_head.weight).view(B, S, -1)
         return out
 
+    def router_aux_loss(self) -> torch.Tensor:
+        """Load-balancing loss of the latest forward over all MoE layers (HF Mixtral's definition and scale)."""
+        layers = [l.mlp for l in self.model.layers if isinstance(l.mlp, MoEMLP)]
+        return load_balancing_loss([m.last_router_logits for m in layers], [m.last_counts for m in layers],
+                                   self.config.num_experts)
+
     # ---- HF interop -------------------------------------------------------------------------------------
     @torch.no_grad()
     def load_hf_state_dict(self, sd: dict, strict: bool = True):
-        """Load a HuggingFace Llama/Qwen2 state dict (separate q/k/v and gate/up projections)."""
+        """Load a HuggingFace Llama/Qwen2 state dict (separate q/k/v and gate/up projections), or a Mixtral one
+        (``mlp.gate.weight``, ``mlp.experts.gate_up_proj``, ``mlp.experts.down_proj``: the same names here)."""
         own = {}
         L = self.config.num_hidden_layers
         g = lambda k: sd[k]
@@ -362,6 +401,10 @@ class LlamaForCausalLM(nn.Module):
                 own[p + "self_attn.qkv_proj.bias"] = torch.cat(
                     [g(p + "self_attn.q_proj.bias"), g(p + "self_attn.k_proj.bias"), g(p + "self_attn.v_proj.bias")], 0)
             own[p + "self_attn.o_proj.weight"] = g(p + "self_attn.o_proj.weight")
+            if self.config.num_experts:
+                for name in ("mlp.gate.weight", "mlp.experts.gate_up_proj", "mlp.experts.down_proj"):
+                    own[p + name] = g(p + name)
+                continue
             own[p + "mlp.gate_up_proj.weight"] = torch.cat([g(p + "mlp.gate_proj.weight"), g(p + "mlp.up_proj.weight")], 0)
             own[p + "mlp.down_proj.weight"] = g(p + "mlp.down_proj.weight")
         return self.load_state_dict(own, strict=strict)

@@ -5,7 +5,10 @@ from .attention import (attention_reference, flash_attn_func, flash_attn_qkvpack
                         flash_attn_xla, get_attention_backend, set_attention_backend, spmd_flash_attn_varlen_xla)
 from .cross_entropy import cross_entropy, fused_linear_cross_entropy
 from .linear import Linear, gemm, linear
-from .liger import apply_liger_kernel, apply_liger_kernel_to_llama, apply_liger_kernel_to_qwen2
+from .liger import (apply_liger_kernel, apply_liger_kernel_to_llama, apply_liger_kernel_to_mixtral,
+                    apply_liger_kernel_to_olmoe, apply_liger_kernel_to_qwen2, apply_liger_kernel_to_qwen2_moe,
+                    apply_liger_kernel_to_qwen3_moe)
+from .moe import MoEMLP, moe_experts, moe_router
 from .optim import FusedAdamW, grad_sqnorm
 from .rmsnorm import RMSNorm, rmsnorm
 from .rope import apply_rope, rope_qkv_, rope_tables

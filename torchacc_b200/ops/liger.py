@@ -93,7 +93,45 @@ def _make_lce_forward(orig_forward):
     return lce_forward
 
 
-def _patch_family(modeling, prefix: str, rms_norm: bool, swiglu: bool, fused_linear_cross_entropy_: bool):
+def _make_moe_lce_forward(orig_forward, modeling):
+    """Causal-LM forward of an HF MoE family with fused linear+CE when labels are given.  The rest is HF's: the router
+    logits are requested from the decoder as HF does, and the family's ``load_balancing_loss_func`` is added with
+    ``router_aux_loss_coef``; the result is a ``MoeCausalLMOutputWithPast`` with ``aux_loss`` and ``router_logits``."""
+
+    def moe_lce_forward(self, input_ids=None, attention_mask=None, position_ids=None, past_key_values=None,
+                        inputs_embeds=None, labels=None, use_cache=None, output_router_logits=None, **kwargs):
+        if labels is None:
+            return orig_forward(self, input_ids=input_ids, attention_mask=attention_mask, position_ids=position_ids,
+                                past_key_values=past_key_values, inputs_embeds=inputs_embeds, use_cache=use_cache,
+                                output_router_logits=output_router_logits, **kwargs)
+        if output_router_logits is None:
+            output_router_logits = self.config.output_router_logits
+        shift = kwargs.pop("shift_labels", None)
+        outputs = self.model(input_ids=input_ids, attention_mask=attention_mask, position_ids=position_ids,
+                             past_key_values=past_key_values, inputs_embeds=inputs_embeds, use_cache=use_cache,
+                             output_router_logits=output_router_logits,
+                             **{k: v for k, v in kwargs.items() if k not in ("num_items_in_batch", "logits_to_keep")})
+        hidden = outputs[0]
+        if shift is None:
+            shift = torch.full_like(labels, -100)
+            shift[..., :-1] = labels[..., 1:]
+        loss = fused_linear_cross_entropy(hidden.reshape(-1, hidden.shape[-1]), self.lm_head.weight,
+                                          shift.reshape(-1))
+        aux_loss = None
+        if output_router_logits:
+            aux_loss = modeling.load_balancing_loss_func(outputs.router_logits, self.num_experts,
+                                                         self.num_experts_per_tok, attention_mask)
+            loss = loss + self.router_aux_loss_coef * aux_loss.to(loss.device)
+        from transformers.modeling_outputs import MoeCausalLMOutputWithPast
+        return MoeCausalLMOutputWithPast(loss=loss, aux_loss=aux_loss, logits=None,
+                                         past_key_values=getattr(outputs, "past_key_values", None),
+                                         router_logits=getattr(outputs, "router_logits", None))
+
+    return moe_lce_forward
+
+
+def _patch_family(modeling, prefix: str, rms_norm: bool, swiglu: bool, fused_linear_cross_entropy_: bool,
+                  moe: bool = False):
     if rms_norm and hasattr(modeling, f"{prefix}RMSNorm"):
         getattr(modeling, f"{prefix}RMSNorm").forward = rms_forward
     if swiglu and hasattr(modeling, f"{prefix}MLP"):
@@ -101,7 +139,7 @@ def _patch_family(modeling, prefix: str, rms_norm: bool, swiglu: bool, fused_lin
     if fused_linear_cross_entropy_ and hasattr(modeling, f"{prefix}ForCausalLM"):
         cls = getattr(modeling, f"{prefix}ForCausalLM")
         if not getattr(cls, "_tb_lce_patched", False):
-            cls.forward = _make_lce_forward(cls.forward)
+            cls.forward = _make_moe_lce_forward(cls.forward, modeling) if moe else _make_lce_forward(cls.forward)
             cls._tb_lce_patched = True
 
 
@@ -122,6 +160,62 @@ def apply_liger_kernel_to_qwen2(rope: bool = True, cross_entropy: bool = False, 
     _patch_family(modeling_qwen2, "Qwen2", rms_norm, swiglu, fused_linear_cross_entropy)
     if rope:
         _patch_rope(modeling_qwen2)
+
+
+def experts_forward(self, hidden_states, top_k_index, top_k_weights):
+    """HF 3-D experts module (``gate_up_proj [E, 2F, H]``, ``down_proj [E, H, F]``) on the grouped GEMM + routing
+    kernels (ops/moe.py).  HF's router and its auxiliary loss stay HF's."""
+    from .moe import moe_experts
+    silu = type(getattr(self, "act_fn", None)).__name__ in ("SiLU", "SiLUActivation")
+    if not (hidden_states.is_cuda and silu and getattr(self, "gate_up_proj_bias", None) is None):
+        return type(self)._tb_orig_forward(self, hidden_states, top_k_index, top_k_weights)
+    return moe_experts(hidden_states, top_k_index, top_k_weights, self.gate_up_proj, self.down_proj)
+
+
+def _patch_experts(modeling, prefix: str) -> None:
+    import inspect
+    cls = getattr(modeling, f"{prefix}Experts", None)
+    if cls is None or getattr(cls, "_tb_orig_forward", None) is not None:
+        return
+    params = inspect.signature(cls.forward).parameters
+    if not all(p in params for p in ("hidden_states", "top_k_index", "top_k_weights")):
+        logger.warning(f"{prefix}Experts.forward has an unknown signature; its experts keep HF's implementation")
+        return
+    cls._tb_orig_forward = cls.forward
+    cls.forward = experts_forward
+
+
+def _moe_family(module_path: str, prefix: str, rms_norm: bool, swiglu: bool, fused_linear_cross_entropy_: bool,
+                experts: bool) -> None:
+    import importlib
+    modeling = importlib.import_module(module_path)
+    _patch_family(modeling, prefix, rms_norm, swiglu, fused_linear_cross_entropy_, moe=True)   # swiglu: shared experts
+    if experts:
+        _patch_experts(modeling, prefix)
+
+
+def apply_liger_kernel_to_mixtral(fused_linear_cross_entropy: bool = True, rms_norm: bool = True, swiglu: bool = True,
+                                  experts: bool = True, **_unused) -> None:
+    _moe_family("transformers.models.mixtral.modeling_mixtral", "Mixtral", rms_norm, swiglu,
+                fused_linear_cross_entropy, experts)
+
+
+def apply_liger_kernel_to_qwen2_moe(fused_linear_cross_entropy: bool = True, rms_norm: bool = True, swiglu: bool = True,
+                                    experts: bool = True, **_unused) -> None:
+    _moe_family("transformers.models.qwen2_moe.modeling_qwen2_moe", "Qwen2Moe", rms_norm, swiglu,
+                fused_linear_cross_entropy, experts)
+
+
+def apply_liger_kernel_to_qwen3_moe(fused_linear_cross_entropy: bool = True, rms_norm: bool = True, swiglu: bool = True,
+                                    experts: bool = True, **_unused) -> None:
+    _moe_family("transformers.models.qwen3_moe.modeling_qwen3_moe", "Qwen3Moe", rms_norm, swiglu,
+                fused_linear_cross_entropy, experts)
+
+
+def apply_liger_kernel_to_olmoe(fused_linear_cross_entropy: bool = True, rms_norm: bool = True, swiglu: bool = True,
+                                experts: bool = True, **_unused) -> None:
+    _moe_family("transformers.models.olmoe.modeling_olmoe", "Olmoe", rms_norm, swiglu, fused_linear_cross_entropy,
+                experts)
 
 
 def _patch_rope(modeling) -> None:
@@ -154,7 +248,11 @@ def apply_liger_kernel(model: Optional[nn.Module] = None) -> None:
         transformers = None
     if transformers is not None:
         families = {"transformers.models.llama.": apply_liger_kernel_to_llama,
-                    "transformers.models.qwen2.": apply_liger_kernel_to_qwen2}
+                    "transformers.models.qwen2.": apply_liger_kernel_to_qwen2,
+                    "transformers.models.mixtral.": apply_liger_kernel_to_mixtral,
+                    "transformers.models.qwen2_moe.": apply_liger_kernel_to_qwen2_moe,
+                    "transformers.models.qwen3_moe.": apply_liger_kernel_to_qwen3_moe,
+                    "transformers.models.olmoe.": apply_liger_kernel_to_olmoe}
         if model is None:
             wanted = list(families.values())
         else:

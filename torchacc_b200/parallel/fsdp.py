@@ -108,7 +108,8 @@ class FlatParamUnit:
                     continue
                 fqn = (mname + "." if mname else "") + pname
                 info = _ParamInfo(sub, pname, fqn, tuple(p.shape), p.numel(), off)
-                info.is_gemm_weight = isinstance(sub, nn.Linear) and pname == "weight"
+                info.is_gemm_weight = ((isinstance(sub, nn.Linear) and pname == "weight")
+                                       or getattr(p, "_tb_gemm_weight", False))   # MoE expert weights (ops/moe.py)
                 # keep every parameter 16-byte aligned inside the flat buffer (TMA / vector loads)
                 off += (p.numel() + 7) // 8 * 8
                 infos.append(info)

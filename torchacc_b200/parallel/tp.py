@@ -333,6 +333,8 @@ def shard_llama_for_tp(lm, tp: TPContext) -> None:
     """Rewrite a native ``LlamaForCausalLM`` in place so each rank keeps 1/tp of the attention heads, the MLP width
     and the lm_head vocabulary."""
     cfg = lm.config
+    if getattr(cfg, "num_experts", 0):
+        raise NotImplementedError("tensor parallelism of mixture-of-experts layers is not supported; use FSDP")
     size, rank = tp.size, tp.rank
     hq, hk, d = cfg.num_attention_heads, cfg.num_key_value_heads, cfg.head_dim
     if hq % size or hk % size:
