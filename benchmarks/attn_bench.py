@@ -28,6 +28,26 @@ def timeit(fn, iters=10, warmup=3):
     return min(ts), sum(ts) / len(ts)
 
 
+def kernel_times(fn, iters=10):
+    """Mean device time per call (ms) of every kernel ``fn`` launches, by kernel name (torch.profiler, no L2 flush)."""
+    from torch.profiler import ProfilerActivity, profile
+    fn()
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            fn()
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        t = getattr(e, "device_time_total", None)
+        if t is None:
+            t = e.cuda_time_total
+        if t > 0:
+            name = e.key.split("(")[0].replace("void ", "").replace("tb::", "")
+            out[name] = out.get(name, 0.0) + t / 1e3 / iters
+    return dict(sorted(out.items(), key=lambda kv: -kv[1]))
+
+
 def device_desc():
     """Card name and power limit (W) of cuda:0, read with nvidia-smi when it is available."""
     desc = {"gpu": torch.cuda.get_device_name(0)}
@@ -50,6 +70,8 @@ def main():
     p.add_argument("--only", default="", help="native: skip the library paths")
     p.add_argument("--deterministic", action="store_true",
                    help="also time the native deterministic backward (deterministic=True)")
+    p.add_argument("--breakdown", action="store_true",
+                   help="per-kernel times of native forward + backward, default and deterministic (torch.profiler)")
     a = p.parse_args()
     from torchacc_b200.ops import attention as A
     B, S, Hq, Hk, D = a.batch, a.seq, a.hq, a.hk, a.d
@@ -77,6 +99,13 @@ def main():
     bench("tb_native", lambda: A.flash_attn_func(q, k, v, causal=True))
     if a.deterministic:
         bench("tb_native_deterministic", lambda: A.flash_attn_func(q, k, v, causal=True, deterministic=True))
+    if a.breakdown:
+        for det in (False, True):
+            def fb():
+                A.flash_attn_func(q, k, v, causal=True, deterministic=det).backward(do)
+            kt = kernel_times(fb)
+            print(json.dumps({"breakdown": "deterministic" if det else "default",
+                              "kernels_ms": {n: round(t, 4) for n, t in kt.items()}}), flush=True)
     dev_desc = device_desc()
     if a.only == "native":
         print(json.dumps({"shape": [B, S, Hq, Hk, D], "device": dev_desc, "results": res}))

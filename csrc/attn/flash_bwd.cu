@@ -1,16 +1,22 @@
 // FlashAttention backward on wgmma / TMA for sm_90a.
 //
-// One CTA per (128-key tile, kv head, batch); it loops over the q heads of the GQA group and over the 64-row query
-// tiles that can see this key tile, so dK/dV are accumulated in registers with no atomics.  Two MMA warpgroups own 64
-// keys each and never wait for one another.  The score tile is computed TRANSPOSED (S^T = K Q^T: accumulator rows =
-// keys, columns = queries), which lets every later GEMM take its operands in place:
+// One CTA per (128-key tile, kv head, batch); it loops over the q heads of the GQA group and over the query tiles that
+// can see this key tile, so dK/dV are accumulated in registers with no atomics.  Query tiles have 128 rows at D = 64
+// and 64 rows at D = 128 (there the 64-register dK and dV accumulators leave no room for 128-column S^T / dP^T tiles)
+// or with dropout (bwd_q_tile).
+// Two MMA warpgroups own 64 keys each.  The score tile is computed TRANSPOSED (S^T = K Q^T: accumulator rows = keys,
+// columns = queries), which lets every later GEMM take its operands in place:
 //   (a) S^T  = K  Q^T    A = K  (smem, K-major)          B = Q  (smem, K-major)
 //   (b) dP^T = V  dO^T   A = V  (smem, K-major)          B = dO (smem, K-major)
 //   in registers:  P^T = exp2(S^T*scale - LSE), dS^T = P^T o (dP^T - delta) * scale
 //   (c) dV  += P^T dO    A = P^T  (registers)            B = dO (smem, MN-major)
 //   (d) dK  += dS^T Q    A = dS^T (registers)            B = Q  (smem, MN-major)
-//   (e) dQ   = dS K      A = dS^T (smem, read MN-major)  B = K  (smem, MN-major), over the warpgroup's 64 keys
-// dQ partial tiles are reduced into the fp32 accumulator with vector red.global.add.
+//   (e) dQ   = dS K      A = dS^T (smem, read MN-major)  B = K  (smem, MN-major), over all 128 keys of the CTA
+// Step (e) reads the dS^T rows of both warpgroups, so it waits on a barrier of the two; each warpgroup then computes a
+// 64 x 64 dQ tile (its half of the query rows at D = 64, its half of the columns at D = 128; with 64-row tiles at
+// D = 64, the partial sum over its own 64 keys), stages it in shared memory while its dV / dK MMAs run, and one thread
+// adds it to the fp32 accumulator with a TMA bulk reduce-add (double-buffered staging).
+// Query rows past the end of the sequence have P = dS = 0, so their rows of the tile add exact zeros.
 // Q/dO tiles stream through a 2-stage TMA ring; K/V stay resident.
 // The deterministic backward compiles step (e) out and computes dQ with flash_bwd_dq_kernel (below) instead.
 //
@@ -27,14 +33,16 @@
 namespace tb {
 
 constexpr int kTile = 128;        // keys per CTA
-constexpr int kQTile = 64;        // query rows per iteration
 constexpr int kBwdThreads = 384;  // producer warpgroup + 2 MMA warpgroups (64 keys each)
 constexpr int kQStages = 2;
+// Query rows per iteration: 128 at D = 64 without dropout.  With dropout the mask state does not fit next to the
+// 128-column S^T / dP^T tiles without spills (the kDQ = false kernel), and the default and deterministic kernels must
+// share the tile so that their dK / dV stay bitwise equal, so both use 64 rows.
+constexpr int bwd_q_tile(int D, bool drop) { return (D == 64 && !drop) ? 128 : 64; }
 
 struct BwdArgs {
   const float* lse;
   const float* delta;
-  float* dq_acc;
   uint16_t* dk;                // bf16 or fp16 (kernel template)
   uint16_t* dv;
   const float* alibi;          // optional ALiBi slopes [Hq] (alibi_bs == 0) or [B, Hq]
@@ -51,24 +59,24 @@ struct BwdArgs {
   long long* trace;   // optional [64 iterations][16 slots] clock64 stamps of CTA (0,0,0) (debug / profiling)
 };
 
-template <int D>
+template <int D, bool kDrop>
 struct BwdSmem {
+  static constexpr int kQTile = bwd_q_tile(D, kDrop);
   static constexpr int kChunks = D / 64;
   static constexpr int kKVBytes = kTile * D * 2;
   static constexpr int kQBytes = kQTile * D * 2;
+  static constexpr int kDQBytes = 64 * 64 * 4;              // one warpgroup's fp32 dQ tile
   static constexpr int kK = 0;
   static constexpr int kV = kK + kKVBytes;
   static constexpr int kQ = kV + kKVBytes;
   static constexpr int kDO = kQ + kQStages * kQBytes;
-  static constexpr int kDS = kDO + kQStages * kQBytes;      // dS^T [128 keys][64 queries], one 128-byte row per key
-  static constexpr int kStat = kDS + kTile * kQTile * 2;    // per warpgroup: lse2[64], delta[64]
+  static constexpr int kDS = kDO + kQStages * kQBytes;      // dS^T: kQTile / 64 chunks of [128 keys][64 queries]
+  static constexpr int kDQ = kDS + kTile * kQTile * 2;      // dQ staging [2 buffers][2 warpgroups], 1024-aligned
+  static constexpr int kStat = kDQ + 2 * 2 * kDQBytes;      // per warpgroup: lse2[kQTile], delta[kQTile]
   static constexpr int kBar = kStat + 2 * 2 * kQTile * 4;
   static constexpr int kTotal = kBar + 128 + 1024;
+  static_assert(kTotal <= 227 * 1024, "backward shared memory exceeds the sm_90 limit");
 };
-
-__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
-  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
-}
 
 // kDQ = false drops step (e) -- the dS^T stores, the dQ MMA and the reduce-adds -- and leaves dK / dV only; the
 // deterministic backward computes dQ afterwards in flash_bwd_dq_kernel.
@@ -76,9 +84,10 @@ template <int D, bool kBf16, bool kDrop, bool kDQ>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
-                 const BwdArgs args) {
-  using S = BwdSmem<D>;
+                 const __grid_constant__ CUtensorMap tmap_dq, const BwdArgs args) {
+  using S = BwdSmem<D, kDrop>;
   constexpr int kChunks = S::kChunks;
+  constexpr int kQTile = S::kQTile;
   constexpr int kQChunk = kQTile * 128;   // bytes of one 64-column chunk of a Q / dO stage
 
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
@@ -115,6 +124,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t sK = base + S::kK, sV = base + S::kV, sQ = base + S::kQ, sDO = base + S::kDO, sDS = base + S::kDS;
+  const uint32_t sDQ = base + S::kDQ;
   float* stat_all = reinterpret_cast<float*>(smem_raw + (base - smem_u32(smem_raw)) + S::kStat);
   const uint32_t bar = base + S::kBar;
   const uint32_t kv_full = bar;
@@ -123,6 +133,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
 
   if (warp_idx == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_q); tma_prefetch_desc(&tmap_k); tma_prefetch_desc(&tmap_v); tma_prefetch_desc(&tmap_do);
+    if constexpr (kDQ) tma_prefetch_desc(&tmap_dq);
   }
   if (warp_idx == 1 && lane == 0) {
     mbar_init(kv_full, 1);
@@ -169,9 +180,17 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const float sl2 = args.scale_log2, sc = args.scale;
   float* stat = stat_all + wg * 2 * kQTile;                           // this warpgroup's copy of lse2 / delta
   const uint32_t sK_w = sK + wg * 8192, sV_w = sV + wg * 8192;        // rows [64 wg, 64 wg + 64) of every 64-column chunk
-  const uint32_t sDS_w = sDS + wg * 8192;
+  // step (e) of this warpgroup: dQ rows [dq_row0, +64) of the query tile, columns [dq_col0, +64), over all 128 keys;
+  // a 64 x 64 tile has nothing to split, so there each warpgroup adds the partial sum over its own 64 keys
+  constexpr bool kDqOwnKeys = kQTile == 64 && D == 64;
+  const int dq_row0 = kQTile == 128 ? 64 * wg : 0, dq_col0 = D == 128 ? 64 * wg : 0;
+  const uint32_t dq_a = sDS + (dq_row0 / 64) * 16384 + (kDqOwnKeys ? wg * 8192 : 0);   // dS^T chunk (and key rows)
+  const uint32_t dq_b = sK + (dq_col0 / 64) * 16384 + (kDqOwnKeys ? wg * 8192 : 0);    // K chunk (and key rows)
   auto wg_sync = [&]() {   // named barrier of this warpgroup
     if (wg == 0) asm volatile("bar.sync 1, 128;" ::: "memory"); else asm volatile("bar.sync 2, 128;" ::: "memory");
+  };
+  auto mma_sync = [&]() {  // named barrier of both MMA warpgroups: step (e) reads the other warpgroup's dS^T rows
+    if constexpr (kDQ) asm volatile("bar.sync 3, 256;" ::: "memory"); else wg_sync();
   };
   const bool tracing = args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
   uint32_t drop_key[2] = {0u, 0u};
@@ -187,18 +206,6 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const int h = iter_head(it), m0 = iter_m0(it);
     const uint32_t q_s = sQ + s * S::kQBytes, do_s = sDO + s * S::kQBytes;
     if (tracing && it < 64) args.trace[it * 16 + 0] = clock64();
-    // row statistics of this query tile (the previous tile's readers are past their dS^T barrier)
-    {
-      const int row = m0 + (tid & 63);
-      const bool ok = row < q_len;
-      const long long off = (long long)h * args.Tq + q_start + row;
-      if (tid < 64) {
-        const float l = ok ? args.lse[off] : INFINITY;
-        stat[tid] = (l == -INFINITY) ? INFINITY : l * 1.4426950408889634f;
-      } else {
-        stat[tid] = ok ? args.delta[off] : 0.f;
-      }
-    }
     mbar_wait(qdo_full(s), (it / kQStages) & 1);
     // ---- (a) S^T = K Q^T, (b) dP^T = V dO^T ----
     float st[kQTile / 2], dpt[kQTile / 2];
@@ -214,7 +221,21 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       wgmma_ss<kQTile, kBf16, 0, 0>(dpt, desc_kmajor_sw128(sV_w + (kk / 4) * 16384, kk % 4),
                                     desc_kmajor_sw128(do_s + (kk / 4) * kQChunk, kk % 4), kk != 0);
     wgmma_commit();
-    wg_sync();            // statistics visible; every thread of the group is done with the previous dS^T tile
+    // row statistics of this query tile, loaded while the MMAs run (the previous tile's readers are past their dS^T
+    // barrier)
+#pragma unroll
+    for (int r = tid; r < 2 * kQTile; r += 128) {   // stat[0, kQTile): lse2, stat[kQTile, 2 kQTile): delta
+      const int row = m0 + (r & (kQTile - 1));
+      const bool ok = row < q_len;
+      const long long off = (long long)h * args.Tq + q_start + row;
+      if (r < kQTile) {
+        const float l = ok ? args.lse[off] : INFINITY;
+        stat[r] = (l == -INFINITY) ? INFINITY : l * 1.4426950408889634f;
+      } else {
+        stat[r] = ok ? args.delta[off] : 0.f;
+      }
+    }
+    mma_sync();           // statistics visible; every reader of the previous dS^T tile is done with it
     wgmma_wait<0>();
     wgmma_fence_acc(st);
     wgmma_fence_acc(dpt);
@@ -268,52 +289,75 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         const uint32_t dsp = pack_h2<kBf16>(ds[0], ds[1]);
         dsfrag[j >> 1][(j & 1) * 2 + i] = dsp;
         if constexpr (kDQ) {
-          // dS^T -> smem row (key), 128B-swizzled: 16-byte unit j of row r lives at unit (j ^ (r & 7))
-          const uint32_t r = (uint32_t)(kr + 8 * i);
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(sDS + r * 128u + (((uint32_t)j ^ (r & 7u)) << 4) + 4u * quad),
+          // dS^T -> smem row (key) of chunk j / 8, 128B-swizzled: 16-byte unit u of row r lives at unit (u ^ (r & 7))
+          const uint32_t r = (uint32_t)(kr + 8 * i), u = (uint32_t)j & 7u;
+          asm volatile("st.shared.b32 [%0], %1;" ::"r"(sDS + (j >> 3) * 16384 + r * 128u + ((u ^ (r & 7u)) << 4) +
+                                                          4u * quad),
                        "r"(dsp)
                        : "memory");
         }
       }
     }
-    if constexpr (kDQ) fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-    wg_sync();
-    // ---- (c) dV += P^T dO, (d) dK += dS^T Q, (e) dQ = dS K over this warpgroup's keys ----
-    float dq[kDQ ? D / 2 : 1];
+    if constexpr (kDQ) {
+      fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
+      // the reduce-add issued two tiles ago has read the staging buffer this tile writes (ordered by the barrier)
+      if (tid == 0) tma_store_wait_read<1>();
+    }
+    mma_sync();
+    // ---- (e) dQ = dS K, then (c) dV += P^T dO, (d) dK += dS^T Q: dQ is its own group, so the dQ tile is staged and
+    // reduced while the tensor cores work on dV / dK ----
+    float dq[kDQ ? 32 : 1];
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
     if constexpr (kDQ) wgmma_fence_acc(dq);
     wgmma_fence();
+    if constexpr (kDQ) {
+#pragma unroll
+      for (int kk = 0; kk < (kDqOwnKeys ? 64 : kTile) / 16; ++kk)
+        wgmma_ss<64, kBf16, 1, 1>(dq, desc_mnmajor_sw128(dq_a, kk, 0), desc_mnmajor_sw128(dq_b, kk, 0), kk != 0);
+      wgmma_commit();
+    }
 #pragma unroll
     for (int kk = 0; kk < kQTile / 16; ++kk)
       wgmma_rs<D, kBf16, 1>(dv, pfrag[kk], desc_mnmajor_sw128(do_s, kk, kQChunk), (it | kk) != 0);
 #pragma unroll
     for (int kk = 0; kk < kQTile / 16; ++kk)
       wgmma_rs<D, kBf16, 1>(dk, dsfrag[kk], desc_mnmajor_sw128(q_s, kk, kQChunk), (it | kk) != 0);
-    if constexpr (kDQ) {
-#pragma unroll
-      for (int kk = 0; kk < 64 / 16; ++kk)
-        wgmma_ss<D, kBf16, 1, 1>(dq, desc_mnmajor_sw128(sDS_w, kk, 0), desc_mnmajor_sw128(sK_w, kk, 16384), kk != 0);
-    }
     wgmma_commit();
+    if constexpr (kDQ) {
+      wgmma_wait<1>();
+      wgmma_fence_acc(dq);
+      // dQ tile -> staging buffer as two [64 rows][32 fp32] halves, 128B-swizzled like the TMA box, then one bulk
+      // reduce-add per half into dq_acc.  Rows past the end of dq_acc are clipped by the tensor map.
+      const uint32_t stg = sDQ + ((it & 1) * 2 + wg) * S::kDQBytes;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const uint32_t r = (warp_idx & 3) * 16 + (lane >> 2) + 8 * i;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {   // columns 8 j + 2 quad, + 1
+          const uint32_t u = 2 * (j & 3) + (quad >> 1);
+          const uint32_t addr = stg + (j >> 2) * 8192 + r * 128 + ((u ^ (r & 7)) << 4) + (quad & 1) * 8;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(dq[4 * j + 2 * i]), "f"(dq[4 * j + 2 * i + 1])
+                       : "memory");
+        }
+      }
+      fence_proxy_async_smem();
+      wg_sync();
+      if (tid == 0) {
+        const int row = q_start + m0 + dq_row0;
+        tma_reduce_add_3d(&tmap_dq, stg, dq_col0, h, row);
+        tma_reduce_add_3d(&tmap_dq, stg + 8192, dq_col0 + 32, h, row);
+        tma_store_commit();
+      }
+    }
     wgmma_wait<0>();
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
-    if constexpr (kDQ) wgmma_fence_acc(dq);
     if (tid == 0) mbar_arrive(qdo_empty(s));
     if (tracing && it < 64) args.trace[it * 16 + 2] = clock64();
-    if constexpr (kDQ) {
-      // dQ rows = queries of the tile: reduce this warpgroup's partial sums into the fp32 accumulator
-      const int qr = (warp_idx & 3) * 16 + (int)(lane >> 2);
-#pragma unroll
-      for (int i = 0; i < 2; ++i) {
-        const int row = m0 + qr + 8 * i;
-        if (row >= q_len) continue;
-        float* dst = args.dq_acc + ((long long)(q_start + row) * args.Hq + h) * D + 2 * quad;
-#pragma unroll
-        for (int j = 0; j < D / 8; ++j) red_add_v2(dst + 8 * j, dq[4 * j + 2 * i], dq[4 * j + 2 * i + 1]);
-      }
-    }
+  }
+  if constexpr (kDQ) {
+    if (tid == 0) tma_store_wait<0>();   // staging buffers stay allocated until the reduce-adds have completed
   }
 
   // ---- epilogue: dV, dK -> bf16 / fp16 ----
@@ -629,11 +673,19 @@ static CUtensorMap make_map_thd_b(const void* base, long long tokens, int heads,
                          strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+// fp32 dQ accumulator [tokens, heads, D]: reduce-add boxes of 64 rows x 32 columns (128 bytes), 128B-swizzled
+static CUtensorMap make_map_dq_acc(float* acc, long long tokens, int heads, int D) {
+  uint64_t dims[3] = {(uint64_t)D, (uint64_t)heads, (uint64_t)tokens};
+  uint64_t strides[2] = {(uint64_t)D * 4, (uint64_t)heads * D * 4};
+  uint32_t box[3] = {32, 1, 64};
+  return make_tensor_map(acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 template <int D, bool kBf16, bool kDrop, bool kDQ>
 static cudaError_t launch_bwd(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
-                              const CUtensorMap& mdo, const BwdArgs& a, int num_k_tiles,
+                              const CUtensorMap& mdo, const CUtensorMap& mdq, const BwdArgs& a, int num_k_tiles,
                               cudaStream_t stream) {
-  using S = BwdSmem<D>;
+  using S = BwdSmem<D, kDrop>;
   auto kern = flash_bwd_kernel<D, kBf16, kDrop, kDQ>;
   static bool configured = false;
   if (!configured) {
@@ -642,7 +694,7 @@ static cudaError_t launch_bwd(const CUtensorMap& mq, const CUtensorMap& mk, cons
     configured = true;
   }
   dim3 grid(num_k_tiles, a.Hk, a.B);
-  kern<<<grid, kBwdThreads, S::kTotal, stream>>>(mq, mk, mv, mdo, a);
+  kern<<<grid, kBwdThreads, S::kTotal, stream>>>(mq, mk, mv, mdo, mdq, a);
   return cudaGetLastError();
 }
 
@@ -711,18 +763,19 @@ cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const
   // 2) main kernel: dK / dV (+ dQ reduce-added into dq_acc unless deterministic)
   cudaError_t e = cudaSuccess;
   if (phases & 2) {
-  CUtensorMap mq, mk, mv, mdo;
+  CUtensorMap mq, mk, mv, mdo, mdq;
   try {
-    mq = make_map_thd_b(q, Tq, Hq, D, q_ts, is_bf16, kQTile);
+    mq = make_map_thd_b(q, Tq, Hq, D, q_ts, is_bf16, bwd_q_tile(D, drop));
     mk = make_map_thd_b(k, Tk, Hk, D, k_ts, is_bf16, kTile);
     mv = make_map_thd_b(v, Tk, Hk, D, v_ts, is_bf16, kTile);
-    mdo = make_map_thd_b(dout, Tq, Hq, D, do_ts, is_bf16, kQTile);
+    mdo = make_map_thd_b(dout, Tq, Hq, D, do_ts, is_bf16, bwd_q_tile(D, drop));
+    mdq = deterministic ? mq : make_map_dq_acc(dq_acc, Tq, Hq, D);   // unused by the deterministic kernel
   } catch (const std::exception& e) {
     fprintf(stderr, "%s\n", e.what());
     return cudaErrorInvalidValue;
   }
   BwdArgs a;
-  a.lse = lse; a.delta = delta; a.dq_acc = deterministic ? nullptr : dq_acc;
+  a.lse = lse; a.delta = delta;
   a.dk = (uint16_t*)dk; a.dv = (uint16_t*)dv;
   a.alibi = alibi_slopes; a.alibi_bs = alibi_batch_stride;
   a.cu_q = cu_q; a.cu_k = cu_k;
@@ -740,8 +793,8 @@ cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const
   const int max_k = cu_k ? (int)Tk : Sk;
   const int num_k_tiles = (max_k + kTile - 1) / kTile;
 #define TB_BWD(DD, BF, DQ)                                                                        \
-  (drop ? launch_bwd<DD, BF, true, DQ>(mq, mk, mv, mdo, a, num_k_tiles, stream)              \
-        : launch_bwd<DD, BF, false, DQ>(mq, mk, mv, mdo, a, num_k_tiles, stream))
+  (drop ? launch_bwd<DD, BF, true, DQ>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream)         \
+        : launch_bwd<DD, BF, false, DQ>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream))
   if (!deterministic) {
     if (is_bf16) e = (D == 128) ? TB_BWD(128, true, true) : TB_BWD(64, true, true);
     else e = (D == 128) ? TB_BWD(128, false, true) : TB_BWD(64, false, true);

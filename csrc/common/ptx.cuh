@@ -179,6 +179,12 @@ TB_DEVICE void tma_reduce_add_2d(const void* desc, uint32_t smem_src, int32_t c0
                "r"(smem_src), "r"(c0), "r"(c1)
                : "memory");
 }
+TB_DEVICE void tma_reduce_add_3d(const void* desc, uint32_t smem_src, int32_t c0, int32_t c1, int32_t c2) {
+  asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(desc)),
+               "r"(smem_src), "r"(c0), "r"(c1), "r"(c2)
+               : "memory");
+}
 // non-tensor bulk copies (contiguous bytes; 16-byte aligned, size % 16 == 0).  Source / destination may be any
 // global address, including a peer GPU's memory mapped over NVLink.
 TB_DEVICE void bulk_load(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
