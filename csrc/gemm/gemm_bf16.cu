@@ -15,6 +15,9 @@
 //                memory, fp32 accumulators in registers (128 per thread; the producer warpgroup hands its registers
 //                over with setmaxnreg), then the epilogue (bias / addend / cast, 16-byte stores after a quad transpose)
 // While the MMA warpgroups run the epilogue of tile i, the producer already fills the ring with tile i+1.
+// Dense launches with nothing to carry run an instantiation without warp 3's role (kCarry == false): the role's
+// function calls (printf, 64-bit division) make ptxas serialise every wgmma of a kernel (warning C7510), so that each
+// m64n256k16 waits for the previous one.  Without them the four wgmmas of a K block are in flight together.
 //
 // Reference parity: replaces the cuBLAS GEMMs the reference reaches through nn.Linear
 // (reference torchacc/__init__.py:97-98 forces XLA onto cuBLAS; eager path uses cuBLASLt).
@@ -240,7 +243,7 @@ __device__ __forceinline__ void tile_coords_sharded(int t, int tiles_m_per_shard
   tn = ln;
 }
 
-template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0, bool kCarry = true>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                  const GemmArgs args) {
@@ -362,8 +365,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
     } else if (warp_idx == 3) {
       // ================================ Carried collective ================================
       // Under static scheduling this warp moves this launch's slice of the pending FSDP all-gather / reduce-scatter
-      // (TMA bulk copies through a private 24 KB ring) while the tiles are computed.
-      if constexpr (kFuse == 0) {
+      // (TMA bulk copies through a private 24 KB ring) while the tiles are computed.  Compiled only into the
+      // instantiations that launches with something to carry use (see kCarry in the header comment).
+      if constexpr (kFuse == 0 && kCarry) {
         if (!args.dynamic && args.carry.slice[0].kind != 0) {
           const uint32_t ring = bar_base + S::kBarrierBytes;
           carry_role(args.carry, ring, ring + kCarryStages * kCarryStageBytes, (int)blockIdx.x, (int)gridDim.x);
@@ -602,11 +606,11 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // ------------------------------------------------------------------------------------------------------
 // Host launcher
 // ------------------------------------------------------------------------------------------------------
-template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0, bool kCarry = true>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, const GemmArgs& args, int num_sms,
                               cudaStream_t stream) {
   using S = GemmSmem;
-  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse, kGroup>;
+  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse, kGroup, kCarry>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotalCarry);
@@ -688,8 +692,11 @@ cudaError_t gemm_bf16_ex(const void* A, const void* B, void* D, const void* bias
   // pending FSDP collectives ride along: bytes proportional to this GEMM's FLOPs (static scheduling only -- under
   // dynamic scheduling the collectives run as their own kernels)
   if (!args.dynamic) carry_take(2.0 * (double)M * (double)N * (double)K, &args.carry);
+  const bool carrying = args.carry.slice[0].kind != 0;
 
-#define TB_DISPATCH(BF, AM, BM) return launch_one<BF, AM, BM, 0>(ta, tbm, args, num_sms, stream)
+#define TB_DISPATCH(BF, AM, BM)                                                 \
+  return carrying ? launch_one<BF, AM, BM, 0>(ta, tbm, args, num_sms, stream) \
+                  : launch_one<BF, AM, BM, 0, 0, false>(ta, tbm, args, num_sms, stream)
 #define TB_MAJORS(BF)                                                  \
   if (!a_mn_major && !b_mn_major) TB_DISPATCH(BF, Major::K, Major::K); \
   if (!a_mn_major && b_mn_major) TB_DISPATCH(BF, Major::K, Major::MN); \
@@ -724,8 +731,12 @@ cudaError_t gemm_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, 
   args.swiglu = 1; args.swiglu_F = F; args.gu_out = GU; args.ldgu = ldgu;
   args.dynamic = 0;
   carry_take(4.0 * (double)M * (double)F * (double)K, &args.carry);
-  if (is_fp16) return launch_one<false, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
-  return launch_one<true, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
+  if (args.carry.slice[0].kind != 0) {
+    if (is_fp16) return launch_one<false, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
+    return launch_one<true, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
+  }
+  if (is_fp16) return launch_one<false, Major::K, Major::K, 0, 0, false>(ta, tbm, args, num_sms, stream);
+  return launch_one<true, Major::K, Major::K, 0, 0, false>(ta, tbm, args, num_sms, stream);
 }
 
 // ------------------------------------------------------------------------------------------------------

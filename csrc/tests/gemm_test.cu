@@ -1,8 +1,10 @@
 // Stand-alone correctness + throughput harness for the wgmma GEMM (no PyTorch).
 //   numerics : every (A-major, B-major, cluster, out dtype, accumulate, bias) combination against cuBLAS fp32-accum
-//   perf     : Llama-3-8B shapes at T=8192 tokens, CUDA-event timed, L2 flushed between iterations,
-//              next to cublasGemmEx on the same buffers.
-// Build: nvcc -gencode arch=compute_90a,code=sm_90a -std=c++17 -O3 csrc/tests/gemm_test.cu csrc/gemm/gemm_bf16.cu -lcublas
+//   perf     : Llama-3-8B shapes and the GEMMs of one bench.py step at T=8192 tokens, CUDA-event timed, L2 flushed
+//              between iterations; static and dynamic tile scheduling and cublasGemmEx on the same buffers.
+// Usage: gemm_test [cluster mask of the numerics: 1, 2 or 3] [perf 0|1] [numerics 0|1]
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -std=c++17 -O3 -I csrc csrc/tests/gemm_test.cu
+//        csrc/gemm/gemm_bf16.cu csrc/fused/carry.cu -lcublas
 #include <cublas_v2.h>
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -101,10 +103,19 @@ static bool check_case(int M, int N, int K, int a_mn, int b_mn, int cluster, int
   return bad == 0;
 }
 
-static void perf_case(cublasHandle_t h, const char* name, int M, int N, int K, int a_mn, int b_mn, int iters) {
+// One shape, three implementations: our kernel under static and under dynamic tile scheduling, and cuBLAS.
+// out_fp32 / accumulate as in the wgrad into an fp32 gradient buffer; swiglu: the gate|up projection with its SwiGLU
+// epilogue (N = 2F; always static; cuBLAS computes the plain GEMM).  Returns the mean times (ms) of the three modes.
+struct PerfResult { float mean[3]; };
+static PerfResult perf_case(cublasHandle_t h, const char* name, int M, int N, int K, int a_mn, int b_mn, int iters,
+                            int out_fp32 = 0, int accumulate = 0, int swiglu = 0) {
+  PerfResult res = {{0.f, 0.f, 0.f}};
   long lda = a_mn ? M : K, ldb = b_mn ? N : K;
-  __nv_bfloat16 *A, *B, *D;
-  CK(cudaMalloc(&A, (size_t)M * K * 2)); CK(cudaMalloc(&B, (size_t)N * K * 2)); CK(cudaMalloc(&D, (size_t)M * N * 2));
+  __nv_bfloat16 *A, *B;
+  void* D;
+  const size_t dbytes = (size_t)M * N * (out_fp32 ? 4 : 2);
+  CK(cudaMalloc(&A, (size_t)M * K * 2)); CK(cudaMalloc(&B, (size_t)N * K * 2)); CK(cudaMalloc(&D, dbytes));
+  CK(cudaMemset(D, 0, dbytes));
   fill_kernel<<<((size_t)M * K + 255) / 256, 256>>>(A, (size_t)M * K, 1u, 1.f);
   fill_kernel<<<((size_t)N * K + 255) / 256, 256>>>(B, (size_t)N * K, 3u, 1.f);
   size_t flush_bytes = 256u << 20;
@@ -113,25 +124,25 @@ static void perf_case(cublasHandle_t h, const char* name, int M, int N, int K, i
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
   double flops = 2.0 * M * N * K;
-  float alpha = 1.f, beta = 0.f;
-  for (int mode = 0; mode < 4; ++mode) {  // 0: ours cluster1, 1: ours cluster2 (dynamic), 2: cuBLAS, 3: cluster2 static
-    if (mode < 2 && !(cl_mask & (1 << mode))) continue;
-    if (mode == 3 && !(cl_mask & 2)) continue;
-    tb::gemm_sched_mode(mode == 3 ? 0 : 1);
+  float alpha = 1.f, beta = accumulate ? 1.f : 0.f;
+  for (int mode = 0; mode < 3; ++mode) {  // 0: ours, static; 1: ours, dynamic; 2: cuBLAS
+    tb::gemm_sched_mode(mode == 1 ? 1 : 0);
     float best = 1e30f, total = 0;
     for (int i = 0; i < iters + 3; ++i) {
       CK(cudaMemsetAsync(flush, i, flush_bytes, 0));  // flush L2 (50 MB) between timed iterations
       cudaEventRecord(e0, 0);
       if (mode != 2) {
-        cudaError_t e = tb::gemm_bf16(A, B, D, nullptr, M, N, K, lda, ldb, N, a_mn, b_mn, false, false,
-                                      mode == 0 ? 1 : 2, num_sms, 0);
+        cudaError_t e = swiglu ? tb::gemm_swiglu_bf16(A, B, D, nullptr, M, N / 2, K, lda, ldb, N / 2, 0, num_sms, 0)
+                               : tb::gemm_bf16(A, B, D, nullptr, M, N, K, lda, ldb, N, a_mn, b_mn, out_fp32,
+                                               accumulate, 1, num_sms, 0);
         if (e != cudaSuccess) { printf("launch failed %s\n", cudaGetErrorString(e)); exit(2); }
       } else {
         // row-major D[M,N] = A_op B_op^T  <=> column-major D^T[N,M] = B_op(cm) * A_op(cm)
         cublasOperation_t opB = b_mn ? CUBLAS_OP_N : CUBLAS_OP_T;  // first operand (B)
         cublasOperation_t opA = a_mn ? CUBLAS_OP_T : CUBLAS_OP_N;  // second operand (A)
         cublasStatus_t st = cublasGemmEx(h, opB, opA, N, M, K, &alpha, B, CUDA_R_16BF, (int)ldb, A, CUDA_R_16BF,
-                                         (int)lda, &beta, D, CUDA_R_16BF, N, CUBLAS_COMPUTE_32F, CUBLAS_GEMM_DEFAULT);
+                                         (int)lda, &beta, D, out_fp32 ? CUDA_R_32F : CUDA_R_16BF, N, CUBLAS_COMPUTE_32F,
+                                         CUBLAS_GEMM_DEFAULT);
         if (st != CUBLAS_STATUS_SUCCESS) { printf("cublas failed %d\n", (int)st); exit(2); }
       }
       cudaEventRecord(e1, 0);
@@ -140,12 +151,14 @@ static void perf_case(cublasHandle_t h, const char* name, int M, int N, int K, i
       cudaEventElapsedTime(&ms, e0, e1);
       if (i >= 3) { total += ms; if (ms < best) best = ms; }
     }
-    const char* mn = mode == 0 ? "tb cluster1" : mode == 1 ? "tb cl2 dyn " : mode == 2 ? "cuBLAS     " : "tb cl2 stat";
-    printf("  %-10s %s M=%d N=%d K=%d : best %.3f ms (%.1f TFLOP/s)  mean %.3f ms (%.1f TFLOP/s)\n", name, mn, M, N, K,
-           best, flops / best * 1e-9, total / iters, flops / (total / iters) * 1e-9);
+    const char* mn = mode == 0 ? "tb stat" : mode == 1 ? "tb dyn " : "cuBLAS ";
+    printf("  %-14s %s M=%6d N=%6d K=%6d : best %7.3f ms (%5.1f TFLOP/s)  mean %7.3f ms (%5.1f TFLOP/s)\n", name, mn, M,
+           N, K, best, flops / best * 1e-9, total / iters, flops / (total / iters) * 1e-9);
+    res.mean[mode] = total / iters;
   }
-  tb::gemm_sched_mode(1);
+  tb::gemm_sched_mode(0);
   cudaFree(A); cudaFree(B); cudaFree(D); cudaFree(flush);
+  return res;
 }
 
 int main(int argc, char** argv) {
@@ -188,6 +201,28 @@ int main(int argc, char** argv) {
     perf_case(h, "wgrad gateup", 28672, 4096, T, 1, 1, 10);
     perf_case(h, "wgrad down", 4096, 14336, T, 1, 1, 10);
     perf_case(h, "square 8k", 8192, 8192, 8192, 0, 0, 10);
+    // the GEMMs of one bench.py step (Llama-3.2-1B: hidden 2048, 32/8 heads of 64, MLP 8192, vocab 128256, 16
+    // layers; 2 x 4096 tokens, gradient checkpointing runs every forward GEMM twice, LM head in 4096-token chunks)
+    printf("== perf (T=8192 tokens, Llama-3.2-1B, the GEMMs of one bench.py step) ==\n");
+    struct Shape { const char* name; int M, N, K, a_mn, b_mn, f32, acc, swiglu, launches; };
+    const int V = 128256;
+    const Shape shapes[] = {
+        {"fwd qkv", T, 3072, 2048, 0, 0, 0, 0, 0, 32},       {"fwd o", T, 2048, 2048, 0, 0, 0, 0, 0, 32},
+        {"fwd gateup", T, 16384, 2048, 0, 0, 0, 0, 1, 32},   {"fwd down", T, 2048, 8192, 0, 0, 0, 0, 0, 32},
+        {"dgrad qkv", T, 2048, 3072, 0, 1, 0, 0, 0, 16},     {"dgrad o", T, 2048, 2048, 0, 1, 0, 0, 0, 16},
+        {"dgrad gateup", T, 2048, 16384, 0, 1, 0, 0, 0, 16}, {"dgrad down", T, 8192, 2048, 0, 1, 0, 0, 0, 16},
+        {"wgrad qkv", 3072, 2048, T, 1, 1, 1, 0, 0, 16},     {"wgrad o", 2048, 2048, T, 1, 1, 1, 0, 0, 16},
+        {"wgrad gateup", 16384, 2048, T, 1, 1, 1, 0, 0, 16}, {"wgrad down", 2048, 8192, T, 1, 1, 1, 0, 0, 16},
+        {"lm logits", 4096, V, 2048, 0, 0, 0, 0, 0, 2},      {"lm dh", 4096, 2048, V, 0, 1, 0, 0, 0, 2},
+        {"lm dW", V, 2048, 4096, 1, 1, 1, 1, 0, 2},
+    };
+    double step_ms[3] = {0, 0, 0};
+    for (const Shape& sh : shapes) {
+      PerfResult r = perf_case(h, sh.name, sh.M, sh.N, sh.K, sh.a_mn, sh.b_mn, 10, sh.f32, sh.acc, sh.swiglu);
+      for (int m = 0; m < 3; ++m) step_ms[m] += (double)r.mean[m] * sh.launches;
+    }
+    printf("GEMM time of one step (mean x launches, L2 flushed): static %.1f ms  dynamic %.1f ms  cuBLAS %.1f ms\n",
+           step_ms[0], step_ms[1], step_ms[2]);
   }
   return ok ? 0 : 1;
 }
