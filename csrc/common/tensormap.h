@@ -64,4 +64,13 @@ inline CUtensorMap make_map_2d_bf16(const void* base, uint64_t rows, uint64_t co
   return make_tensor_map(base, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
+// 2-D fp32 matrix [rows][cols] (cols contiguous, row pitch ld elements), SWIZZLE_128B boxes (box_cols <= 32).
+inline CUtensorMap make_map_2d_f32(const void* base, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_cols,
+                                   uint32_t box_rows) {
+  uint64_t dims[2] = {cols, rows};
+  uint64_t strides[1] = {ld * 4};
+  uint32_t box[2] = {box_cols, box_rows};
+  return make_tensor_map(base, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 }  // namespace tb

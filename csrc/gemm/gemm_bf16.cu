@@ -15,6 +15,9 @@
 //                memory, fp32 accumulators in registers (128 per thread; the producer warpgroup hands its registers
 //                over with setmaxnreg), then the epilogue (bias / addend / cast, 16-byte stores after a quad transpose)
 // While the MMA warpgroups run the epilogue of tile i, the producer already fills the ring with tile i+1.
+// Dense launches with aligned outputs and nothing to carry stage the epilogue instead (kStaged): fragments go to
+// 128B-swizzled shared-memory boxes that one thread per warpgroup stores (or reduce-adds) with TMA, and a 16-bit
+// addend arrives in those boxes by TMA, so the MMA warpgroups never wait on global memory between two tiles.
 // Dense launches with nothing to carry run an instantiation without warp 3's role (kCarry == false): the role's
 // function calls (printf, 64-bit division) make ptxas serialise every wgmma of a kernel (warning C7510), so that each
 // m64n256k16 waits for the previous one.  Without them the four wgmmas of a K block are in flight together.
@@ -219,6 +222,10 @@ struct GemmSmem {
   static constexpr int kBarrierBytes = 1024;
   static constexpr int kTotal = kStages * kStageBytes + kBarrierBytes + 1024;  // +1024 alignment slack
   static constexpr int kTotalCarry = kTotal + kCarrySmemBytes;                 // + the copy warp's private ring
+  // staged epilogue: two 8 KB buffers per MMA warpgroup, each one 128B-swizzled TMA box of 64 rows x 128 bytes
+  static constexpr int kStagingBytes = 2 * 2 * 8192;
+  static constexpr int kTotalStaged = kTotal + kStagingBytes;
+  static_assert(kTotalStaged <= 227 * 1024, "staging does not fit next to the ring");
 };
 
 __device__ __forceinline__ void tile_coords(int t, int num_m_tiles, int num_n_tiles, int& tm, int& tn) {
@@ -243,14 +250,21 @@ __device__ __forceinline__ void tile_coords_sharded(int t, int tiles_m_per_shard
   tn = ln;
 }
 
-template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0, bool kCarry = true>
+// Tensor maps of the staged epilogue (kStaged): D (16-bit: 64 x 64 boxes, fp32: 32 x 64), the 16-bit addend C, and
+// the SwiGLU pre-activation g|u.  Unused maps are left zeroed.
+struct EpiMaps {
+  CUtensorMap d, c, gu;
+};
+
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0, bool kCarry = true, bool kStaged = false>
 __global__ void __launch_bounds__(kNumThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                 const GemmArgs args) {
+                 const GemmArgs args, const __grid_constant__ EpiMaps maps) {
   using S = GemmSmem;
   constexpr int kStages = S::kStages;
   constexpr int kTA = (kAMajor == Major::MN) ? 1 : 0, kTB = (kBMajor == Major::MN) ? 1 : 0;
   static_assert(kGroup == 0 || kFuse == 0, "grouped GEMMs are not fused with collectives");
+  static_assert(!kStaged || (kFuse == 0 && kGroup == 0 && !kCarry), "the staged epilogue is for plain dense launches");
   static_assert(kGroup != 2 || (kAMajor == Major::MN && kBMajor == Major::MN), "grouped wgrad reads both operands MN-major");
 
   extern __shared__ uint8_t smem_raw[];
@@ -305,11 +319,19 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
   if (warp_idx == 0 && lane == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if constexpr (kStaged) {
+      tma_prefetch_desc(&maps.d);
+      if (args.C != nullptr && !args.out_fp32) tma_prefetch_desc(&maps.c);
+      if (args.gu_out != nullptr) tma_prefetch_desc(&maps.gu);
+    }
   }
   if (warp_idx == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 2);   // one arrival per MMA warpgroup
+    }
+    if constexpr (kStaged) {
+      for (int b = 0; b < 4; ++b) mbar_init(bar_base + 8u * (2 * kStages + b), 1);   // addend loads, see below
     }
     fence_mbar_init();
   }
@@ -405,6 +427,20 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
         }
       }
     };
+    // Staged epilogue (kStaged): each warpgroup writes its 64 rows chunk by chunk into one of its two 8 KB staging
+    // buffers (128B-swizzled, one TMA box each), and one elected thread stores the box with TMA while the warpgroup
+    // fills the other buffer and then goes back to the next tile's wgmmas.  A 16-bit addend is loaded into the buffers
+    // by TMA behind mbarriers (the first two chunks during the tile's mainloop), an fp32 accumulation (C == D) is
+    // issued as a TMA reduce-add, so the epilogue loads nothing from global memory but the bias.
+    const uint32_t stage_buf = bar_base + S::kBarrierBytes + wg * 16384;   // + b * 8192, b = chunk & 1
+    const bool wg_leader = (threadIdx.x & 127) == 0;
+    const bool stage_addend = kStaged && args.C != nullptr && !args.out_fp32;   // fp32 C is always C == D (host)
+    auto cload_bar = [&](int b) { return bar_base + 8u * (2 * kStages + 2 * wg + b); };
+    auto load_addend = [&](int chunk, int tm, int tn) {   // wg_leader only, buffer (chunk & 1) free
+      const int b = chunk & 1;
+      mbar_arrive_expect_tx(cload_bar(b), 8192);
+      tma_load_2d(stage_buf + b * 8192, &maps.c, cload_bar(b), tn * kBlockN + 64 * chunk, tm * kBlockM + wg * 64);
+    };
     int it = 0;
     for (int t = cta; t < num_tiles; t += num_ctas) {
       int tm, tn, shard;
@@ -445,12 +481,153 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
           wgmma_wait<1>();
           if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar((it - 1) % kStages));
         }
+        if constexpr (kStaged) {
+          // addend chunks 0 and 1 of this tile, once the previous tile's stores have left the staging buffers
+          if (stage_addend && wg_leader && kb == min(nkb - 1, 1)) {
+            tma_store_wait_read<0>();
+            load_addend(0, tm, tn);
+            load_addend(1, tm, tn);
+          }
+        }
       }
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       if ((threadIdx.x & 127) == 0) mbar_arrive(empty_bar((it - 1) % kStages));
 
       const long long row0 = (long long)tm * kBlockM + frag_row;   // this thread's rows: row0 and row0 + 8
+      if constexpr (kStaged) {
+        // Fragment element (row r + 8 half, column 8 j + 2 quad + e) of the warpgroup's 64 rows.  A 16-bit chunk is
+        // 64 columns (j in [8c, 8c + 8)): each pair is one 32-bit word in 16-byte unit j % 8 of its 128-byte row.  An
+        // fp32 chunk is 32 columns (j in [4c, 4c + 4)): each pair is 8 bytes in unit 2 (j % 4) + quad / 2.  The
+        // 128-byte swizzle XORs the unit with the row's index mod 8.
+        const uint32_t r = (uint32_t)(wq * 16) + (lane >> 2);
+        auto addr16 = [&](int b, int jj, int half) {
+          const uint32_t row = r + 8u * half;
+          return stage_buf + b * 8192 + row * 128u + (((uint32_t)jj ^ (row & 7u)) << 4) + quad * 4u;
+        };
+        auto addr32 = [&](int b, int jj, int half) {
+          const uint32_t row = r + 8u * half;
+          return stage_buf + b * 8192 + row * 128u + (((uint32_t)(2 * jj) + (quad >> 1)) ^ (row & 7u)) * 16u +
+                 (quad & 1u) * 8u;
+        };
+        const int mrow = tm * kBlockM + wg * 64;
+        auto wg_sync = [&]() { named_bar_sync(1 + wg, 128); };
+        auto acquire = [&]() {   // this chunk's buffer is free again: the store two chunks back has read it
+          if (wg_leader) tma_store_wait_read<1>();
+          wg_sync();
+        };
+        auto release = [&]() {   // generic-proxy writes -> visible to the TMA store, all 128 threads done
+          fence_proxy_async_smem();
+          wg_sync();
+        };
+        auto store16 = [&](const CUtensorMap* map, int b, int col) {
+          release();
+          if (wg_leader) {
+            tma_store_2d(map, stage_buf + b * 8192, col, mrow);
+            tma_store_commit();
+          }
+        };
+        if (args.swiglu) {
+          // h chunks 0, 1, then (with gu_out) g chunks 0, 1 and u chunks 0, 1; same arithmetic as the register path
+          const int hcol = tn * (kBlockN / 2);
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            acquire();
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * c + jj;
+#pragma unroll
+              for (int half = 0; half < 2; ++half) {
+                float hv[2];
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float gt = acc[4 * j + 2 * half + e], up = acc[4 * (j + 16) + 2 * half + e];
+                  float th;
+                  asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * gt));
+                  hv[e] = gt * fmaf(0.5f, th, 0.5f) * up;
+                }
+                st_shared_b32(addr16(c, jj, half), pk(hv[0], hv[1]));
+              }
+            }
+            store16(&maps.d, c, hcol + 64 * c);
+          }
+          if (args.gu_out != nullptr) {
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {   // c < 2: gate columns, c >= 2: up columns (accumulator columns + 128)
+              const int b = c & 1, jo = (c >> 1) * 16 + 8 * b;
+              acquire();
+#pragma unroll
+              for (int jj = 0; jj < 8; ++jj)
+#pragma unroll
+                for (int half = 0; half < 2; ++half)
+                  st_shared_b32(addr16(b, jj, half), pk(acc[4 * (jo + jj) + 2 * half], acc[4 * (jo + jj) + 2 * half + 1]));
+              store16(&maps.gu, b, (c >> 1) * args.swiglu_F + hcol + 64 * b);
+            }
+          }
+          continue;
+        }
+        const int n0 = tn * kBlockN;
+        const uint16_t* bias = reinterpret_cast<const uint16_t*>(args.bias);
+        if (args.out_fp32) {
+          // fp32: 8 chunks of 32 columns; accumulation (C == D) adds the staged tile with a TMA reduce-add, which is
+          // old + (acc + b) where the register path computes (acc + b) + old: the same IEEE sum
+#pragma unroll
+          for (int c = 0; c < 8; ++c) {
+            const int b = c & 1;
+            acquire();
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = 4 * c + jj;
+              const int col = n0 + 8 * j + 2 * (int)quad;
+              const float b0 = (bias && col < args.N) ? ld1(bias + col) : 0.f;
+              const float b1 = (bias && col + 1 < args.N) ? ld1(bias + col + 1) : 0.f;
+#pragma unroll
+              for (int half = 0; half < 2; ++half)
+                st_shared_v2_f32(addr32(b, jj, half), acc[4 * j + 2 * half] + b0, acc[4 * j + 2 * half + 1] + b1);
+            }
+            release();
+            if (wg_leader) {
+              if (args.C != nullptr) tma_reduce_add_2d(&maps.d, stage_buf + b * 8192, n0 + 32 * c, mrow);
+              else tma_store_2d(&maps.d, stage_buf + b * 8192, n0 + 32 * c, mrow);
+              tma_store_commit();
+            }
+          }
+          continue;
+        }
+        // 16-bit: 4 chunks of 64 columns; bias and addend in fp32 in the accumulator layout, then one rounding
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int b = c & 1;
+          if (stage_addend) mbar_wait(cload_bar(b), (c >> 1) & 1);
+          else acquire();
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = 8 * c + jj;
+            const int col = n0 + 8 * j + 2 * (int)quad;
+            float b0 = 0.f, b1 = 0.f;
+            if (bias) {
+              if (col < args.N) b0 = ld1(bias + col);
+              if (col + 1 < args.N) b1 = ld1(bias + col + 1);
+            }
+#pragma unroll
+            for (int half = 0; half < 2; ++half) {
+              float v0 = acc[4 * j + 2 * half], v1 = acc[4 * j + 2 * half + 1];
+              if (bias) { v0 += b0; v1 += b1; }
+              if (stage_addend) {
+                const float2 old = unpack_h2<kBf16>(ld_shared_b32(addr16(b, jj, half)));
+                v0 += old.x; v1 += old.y;
+              }
+              st_shared_b32(addr16(b, jj, half), pk(v0, v1));
+            }
+          }
+          store16(&maps.d, b, n0 + 64 * c);
+          if (stage_addend && wg_leader && c + 2 < 4) {   // addend chunk c + 2 into this buffer once it is read out
+            tma_store_wait_read<0>();
+            load_addend(c + 2, tm, tn);
+          }
+        }
+        continue;
+      }
       if constexpr (kFuse == 2) {
         // bf16 partial tile -> staging slot [my rank] of the rank that owns this row block (peer stores over NVLink,
         // 16 bytes per lane after the quad transpose); slots are row-major [rows_per_rank][N padded to the tile].
@@ -597,6 +774,9 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
       }
     }
     flush_arrivals();
+    if constexpr (kStaged) {
+      if (wg_leader) tma_store_wait<0>();   // the staging buffers must outlive the stores that read them
+    }
   }
   if constexpr (kFuse == 0) {
     if (args.carry.debug != nullptr && blockIdx.x == 0 && threadIdx.x == 0) args.carry.debug[7] = carry_now_ns();
@@ -606,14 +786,15 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 // ------------------------------------------------------------------------------------------------------
 // Host launcher
 // ------------------------------------------------------------------------------------------------------
-template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0, bool kCarry = true>
+template <bool kBf16, Major kAMajor, Major kBMajor, int kFuse, int kGroup = 0, bool kCarry = true, bool kStaged = false>
 static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, const GemmArgs& args, int num_sms,
-                              cudaStream_t stream) {
+                              cudaStream_t stream, const EpiMaps& maps = EpiMaps{}) {
   using S = GemmSmem;
-  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse, kGroup, kCarry>;
+  auto kern = gemm_bf16_kernel<kBf16, kAMajor, kBMajor, kFuse, kGroup, kCarry, kStaged>;
   static bool configured = false;
   if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotalCarry);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         kStaged ? S::kTotalStaged : S::kTotalCarry);
     if (e != cudaSuccess) return e;
     configured = true;
   }
@@ -626,8 +807,9 @@ static cudaError_t launch_one(const CUtensorMap& ta, const CUtensorMap& tb_, con
   if (ctas < 1) ctas = 1;
   ctas += comm_ctas;
   if (kFuse == 0 && args.dynamic) ctas = num_tiles;   // one CTA per tile: the block scheduler hands them to free SMs
-  const int smem = carrying ? S::kTotalCarry : S::kTotal;   // the ring only when there is something to carry
-  kern<<<ctas, kNumThreads, smem, stream>>>(ta, tb_, args);
+  // the copy warp's ring only when there is something to carry, the staging buffers only for the staged epilogue
+  const int smem = kStaged ? S::kTotalStaged : (carrying ? S::kTotalCarry : S::kTotal);
+  kern<<<ctas, kNumThreads, smem, stream>>>(ta, tb_, args, maps);
   return cudaGetLastError();
 }
 
@@ -693,10 +875,30 @@ cudaError_t gemm_bf16_ex(const void* A, const void* B, void* D, const void* bias
   // dynamic scheduling the collectives run as their own kernels)
   if (!args.dynamic) carry_take(2.0 * (double)M * (double)N * (double)K, &args.carry);
   const bool carrying = args.carry.slice[0].kind != 0;
+  // The staged (TMA) epilogue needs D and C 16-byte aligned with row pitches of whole 16 bytes; an fp32 addend is
+  // only staged as an accumulation (C == D, TMA reduce-add).  Everything else keeps the register epilogue.
+  const long long esz = out_fp32 ? 4 : 2;
+  auto aligned = [&](const void* p, long long ld) { return reinterpret_cast<uintptr_t>(p) % 16 == 0 && (ld * esz) % 16 == 0; };
+  const bool staged = !carrying && aligned(D, ldd) &&
+                      (C == nullptr || (out_fp32 ? (C == D && ldc == ldd) : aligned(C, ldc)));
+  EpiMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  if (staged) {
+    try {
+      maps.d = out_fp32 ? make_map_2d_f32(D, M, N, ldd, 32, 64) : make_map_2d_bf16(D, M, N, ldd, 64, 64);
+      if (C != nullptr && !out_fp32) maps.c = make_map_2d_bf16(C, M, N, ldc, 64, 64);
+    } catch (const std::exception& e) {
+      fprintf(stderr, "%s\n", e.what());
+      return cudaErrorInvalidValue;
+    }
+  }
 
-#define TB_DISPATCH(BF, AM, BM)                                                 \
-  return carrying ? launch_one<BF, AM, BM, 0>(ta, tbm, args, num_sms, stream) \
-                  : launch_one<BF, AM, BM, 0, 0, false>(ta, tbm, args, num_sms, stream)
+#define TB_DISPATCH(BF, AM, BM)                                                                       \
+  {                                                                                                   \
+    if (carrying) return launch_one<BF, AM, BM, 0>(ta, tbm, args, num_sms, stream);                   \
+    if (staged) return launch_one<BF, AM, BM, 0, 0, false, true>(ta, tbm, args, num_sms, stream, maps); \
+    return launch_one<BF, AM, BM, 0, 0, false>(ta, tbm, args, num_sms, stream);                       \
+  }
 #define TB_MAJORS(BF)                                                  \
   if (!a_mn_major && !b_mn_major) TB_DISPATCH(BF, Major::K, Major::K); \
   if (!a_mn_major && b_mn_major) TB_DISPATCH(BF, Major::K, Major::MN); \
@@ -735,8 +937,18 @@ cudaError_t gemm_swiglu_bf16(const void* A, const void* Wgu, void* H, void* GU, 
     if (is_fp16) return launch_one<false, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
     return launch_one<true, Major::K, Major::K, 0>(ta, tbm, args, num_sms, stream);
   }
-  if (is_fp16) return launch_one<false, Major::K, Major::K, 0, 0, false>(ta, tbm, args, num_sms, stream);
-  return launch_one<true, Major::K, Major::K, 0, 0, false>(ta, tbm, args, num_sms, stream);
+  // H and g|u are 16-byte aligned with whole-16-byte pitches (checked above): always the staged epilogue
+  EpiMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  try {
+    maps.d = make_map_2d_bf16(H, M, F, ldh, 64, 64);
+    if (GU != nullptr) maps.gu = make_map_2d_bf16(GU, M, 2 * (uint64_t)F, ldgu, 64, 64);
+  } catch (const std::exception& e) {
+    fprintf(stderr, "%s\n", e.what());
+    return cudaErrorInvalidValue;
+  }
+  if (is_fp16) return launch_one<false, Major::K, Major::K, 0, 0, false, true>(ta, tbm, args, num_sms, stream, maps);
+  return launch_one<true, Major::K, Major::K, 0, 0, false, true>(ta, tbm, args, num_sms, stream, maps);
 }
 
 // ------------------------------------------------------------------------------------------------------
