@@ -16,7 +16,7 @@ template <typename T>
 static inline T* P(uint64_t p) { return reinterpret_cast<T*>(p); }
 
 TB_API const char* tb_error_string(int code) { return cudaGetErrorString(static_cast<cudaError_t>(code)); }
-TB_API int tb_abi_version() { return 3; }
+TB_API int tb_abi_version() { return 4; }
 
 TB_API int tb_device_info(int device, int* num_sms, int* cc_major, int* cc_minor, long long* smem_optin) {
   cudaDeviceProp prop;
@@ -85,10 +85,10 @@ TB_API int tb_cross_entropy(uint64_t logits, uint64_t labels, uint64_t loss_rows
 }
 TB_API int tb_adamw_flat(uint64_t p, uint64_t g, int grad_is_bf16, uint64_t m, uint64_t v, uint64_t p_lp, long long n,
                          float lr, float beta1, float beta2, float eps, float weight_decay, int step,
-                         uint64_t grad_scale, uint64_t found_inf, int num_sms, uint64_t stream) {
+                         uint64_t skipped, uint64_t grad_scale, uint64_t found_inf, int num_sms, uint64_t stream) {
   return (int)tb::adamw_flat(P<float>(p), P<void>(g), grad_is_bf16 != 0, P<float>(m), P<float>(v), P<void>(p_lp), n,
-                             lr, beta1, beta2, eps, weight_decay, step, P<float>(grad_scale), P<float>(found_inf),
-                             num_sms, S(stream));
+                             lr, beta1, beta2, eps, weight_decay, step, P<int>(skipped), P<float>(grad_scale),
+                             P<float>(found_inf), num_sms, S(stream));
 }
 TB_API int tb_sqnorm_accumulate(uint64_t g, int is_bf16, long long n, uint64_t out, float pre_scale, int num_sms,
                                 uint64_t stream) {

@@ -307,6 +307,16 @@ TB_DEVICE float fast_exp2(float x) {
   asm volatile("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
+// sigmoid(x) = 1 / (1 + 2^(-x log2 e)) with MUFU ex2 and rcp: a few fp32 ulps of relative error over the whole range,
+// also for x << 0 where sigmoid(x) itself is tiny.  (0.5 + 0.5 tanh.approx(x / 2) is one MUFU op, but tanh.approx has
+// about 2^-11 relative error, which near tanh = -1 is an absolute sigmoid error larger than sigmoid(x) for x < -8.)
+// Large negative x: 2^(-x log2 e) overflows to +inf and the reciprocal gives 0.
+TB_DEVICE float fast_sigmoid(float x) {
+  float e, r;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(x * -1.4426950408889634f));
+  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.f + e));
+  return r;
+}
 
 template <typename T>
 TB_DEVICE T warp_reduce_sum(T v) {

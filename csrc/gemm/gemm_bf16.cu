@@ -542,9 +542,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                   const float gt = acc[4 * j + 2 * half + e], up = acc[4 * (j + 16) + 2 * half + e];
-                  float th;
-                  asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * gt));
-                  hv[e] = gt * fmaf(0.5f, th, 0.5f) * up;
+                  hv[e] = gt * fast_sigmoid(gt) * up;
                 }
                 st_shared_b32(addr16(c, jj, half), pk(hv[0], hv[1]));
               }
@@ -669,9 +667,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_consta
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                   const float gt = acc[4 * j + 2 * half + e], up = acc[4 * (j + 16) + 2 * half + e];
-                  float th;
-                  asm("tanh.approx.f32 %0, %1;" : "=f"(th) : "f"(0.5f * gt));     // sigmoid(g) = 0.5 + 0.5 tanh(g / 2)
-                  hv[e] = gt * fmaf(0.5f, th, 0.5f) * up;
+                  hv[e] = gt * fast_sigmoid(gt) * up;
                 }
                 xh[jj] = pk(hv[0], hv[1]);
                 xg[jj] = pk(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);

@@ -5,7 +5,8 @@
 //   chunked lm_head GEMM in Python this is the fused-linear-cross-entropy of reference ops/liger.py:72-76.
 // * adamw_flat: one pass over the local fp32 master shard: reads grad (bf16 or fp32), m, v, p; applies the
 //   device-resident scale (clip coefficient x 1/loss_scale, no host sync) and the found_inf skip; writes p, m, v
-//   and the bf16 compute copy that the next all-gather sends.  Replaces torch fused Adam / torch_xla syncfree
+//   and the bf16 compute copy that the next all-gather sends.  A skipped step is counted on the device, so it does
+//   not advance the bias correction (as in torch's fused AdamW).  Replaces torch fused Adam / torch_xla syncfree
 //   optimizers (reference utils/patch.py:55-58).
 #include "../common/ptx.cuh"
 #include "ops.h"
@@ -33,7 +34,8 @@ cross_entropy_kernel(__nv_bfloat16* __restrict__ logits, const long long* __rest
   const bool ignored = label == ignore_index;
   const int nvec = V >> 3;
   const float kLog2e = 1.4426950408889634f;
-  // pass 1: online softmax statistics
+  // pass 1: online softmax statistics.  While every logit a thread has seen is -inf (masked), its running max stays
+  // -inf and nothing is added: (-inf) - (-inf) would be NaN and poison the running sum for the rest of the row.
   float m = -INFINITY, s = 0.f;
   for (int v = threadIdx.x; v < nvec; v += kCEThreads) {
     float f[8];
@@ -42,6 +44,7 @@ cross_entropy_kernel(__nv_bfloat16* __restrict__ logits, const long long* __rest
 #pragma unroll
     for (int j = 1; j < 8; ++j) lm = fmaxf(lm, f[j]);
     const float nm = fmaxf(m, lm);
+    if (nm == -INFINITY) continue;
     float acc = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc += fast_exp2((f[j] - nm) * kLog2e);
@@ -51,6 +54,7 @@ cross_entropy_kernel(__nv_bfloat16* __restrict__ logits, const long long* __rest
   for (int i = nvec * 8 + threadIdx.x; i < V; i += kCEThreads) {  // tail (V % 8 != 0)
     const float f = __bfloat162float(lr[i]);
     const float nm = fmaxf(m, f);
+    if (nm == -INFINITY) continue;
     s = s * fast_exp2((m - nm) * kLog2e) + fast_exp2((f - nm) * kLog2e);
     m = nm;
   }
@@ -120,9 +124,18 @@ template <typename GradT>
 __global__ void __launch_bounds__(256)
 adamw_kernel(float* __restrict__ p, const GradT* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
              __nv_bfloat16* __restrict__ p_lp, long long n, float lr, float beta1, float beta2, float eps,
-             float weight_decay, float bc1, float bc2_sqrt, const float* __restrict__ grad_scale,
-             const float* __restrict__ found_inf) {
-  if (found_inf && *found_inf != 0.f) return;  // skipped step (fp16 loss scaling)
+             float weight_decay, int step, float bc1, float bc2_sqrt, int* __restrict__ skipped,
+             const float* __restrict__ grad_scale, const float* __restrict__ found_inf) {
+  if (found_inf && *found_inf != 0.f) {        // skipped step (fp16 loss scaling)
+    // only a skipped launch writes the counter and only a running launch reads it, so one thread may bump it
+    if (skipped && blockIdx.x == 0 && threadIdx.x == 0) *skipped += 1;
+    return;
+  }
+  if (skipped) {                                // bias correction of the steps actually taken
+    const double t = (double)(step - *skipped);
+    bc1 = (float)(1.0 - pow((double)beta1, t));
+    bc2_sqrt = (float)sqrt(1.0 - pow((double)beta2, t));
+  }
   const float gs = grad_scale ? *grad_scale : 1.f;
   const long long nvec = n >> 2;
   const float step_size = lr / bc1;
@@ -194,7 +207,7 @@ adamw_kernel(float* __restrict__ p, const GradT* __restrict__ g, float* __restri
 }
 
 cudaError_t adamw_flat(float* p, const void* g, bool grad_is_bf16, float* m, float* v, void* p_lp, long long n,
-                       float lr, float beta1, float beta2, float eps, float weight_decay, int step,
+                       float lr, float beta1, float beta2, float eps, float weight_decay, int step, int* skipped,
                        const float* grad_scale, const float* found_inf, int num_sms, cudaStream_t stream) {
   if (n == 0) return cudaSuccess;
   const float bc1 = 1.f - powf(beta1, (float)step);
@@ -204,11 +217,12 @@ cudaError_t adamw_flat(float* p, const void* g, bool grad_is_bf16, float* m, flo
   int grid = (int)(blocks < (long long)num_sms * 16 ? blocks : (long long)num_sms * 16);
   if (grad_is_bf16)
     adamw_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(p, (const __nv_bfloat16*)g, m, v, (__nv_bfloat16*)p_lp, n,
-                                                          lr, beta1, beta2, eps, weight_decay, bc1, bc2_sqrt,
-                                                          grad_scale, found_inf);
+                                                          lr, beta1, beta2, eps, weight_decay, step, bc1, bc2_sqrt,
+                                                          skipped, grad_scale, found_inf);
   else
     adamw_kernel<float><<<grid, 256, 0, stream>>>(p, (const float*)g, m, v, (__nv_bfloat16*)p_lp, n, lr, beta1, beta2,
-                                                  eps, weight_decay, bc1, bc2_sqrt, grad_scale, found_inf);
+                                                  eps, weight_decay, step, bc1, bc2_sqrt, skipped, grad_scale,
+                                                  found_inf);
   return cudaGetLastError();
 }
 

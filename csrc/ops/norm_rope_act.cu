@@ -295,17 +295,9 @@ cudaError_t rope_inplace(void* x, const float* cos_t, const float* sin_t, const 
 
 // ---------------------------------------------------------------------------------------------------
 // SwiGLU: h = silu(g) * u.  g and u are separate row-strided matrices [T, F] (for the fused gate|up projection
-// u = g + F and both strides are 2F); h is [T, F] contiguous.
+// u = g + F and both strides are 2F); h is [T, F] contiguous.  sigmoid is fast_sigmoid (common/ptx.cuh): ex2 + rcp,
+// no IEEE divide and its fix-up code.
 // ---------------------------------------------------------------------------------------------------
-// sigmoid through ONE MUFU op: sigmoid(x) = 0.5 + 0.5 * tanh(0.5 x)  (tanh.approx.f32, rel. error 2^-11 -- far below
-// the bf16 rounding of the result; exp + divide would be two MUFU ops plus the divide's fix-up code and makes the
-// kernel issue-bound instead of HBM-bound).
-TB_DEVICE float fast_sigmoid(float x) {
-  float t;
-  asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(0.5f * x));
-  return fmaf(0.5f, t, 0.5f);
-}
-
 // One CTA walks whole rows (no per-element index division); two independent 16-byte vector pairs per thread and
 // iteration keep 4 loads in flight per thread.
 template <bool kBf16>

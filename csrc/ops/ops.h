@@ -21,8 +21,10 @@ cudaError_t swiglu_bwd(const void* dh, const void* g, const void* u, void* dg, v
 cudaError_t cross_entropy_fwd_bwd(void* logits, const long long* labels, float* loss_rows, float* lse_rows, int n,
                                   int V, long long ld, int ignore_index, const float* scale_ptr, float scale_val,
                                   bool write_grad, cudaStream_t stream);
+// step counts every call; skipped (optional, int32 device counter) counts the calls that found_inf skipped.  With it
+// the bias correction uses step - *skipped, computed on the device; without it, step (computed on the host).
 cudaError_t adamw_flat(float* p, const void* g, bool grad_is_bf16, float* m, float* v, void* p_lp, long long n,
-                       float lr, float beta1, float beta2, float eps, float weight_decay, int step,
+                       float lr, float beta1, float beta2, float eps, float weight_decay, int step, int* skipped,
                        const float* grad_scale, const float* found_inf, int num_sms, cudaStream_t stream);
 cudaError_t sqnorm_accumulate(const void* g, bool is_bf16, long long n, float* out, float pre_scale, int num_sms,
                               cudaStream_t stream);

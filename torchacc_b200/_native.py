@@ -32,7 +32,7 @@ _SIGS = {
     "tb_swiglu_fwd": ([u64, u64, u64, i64, i32, i64, i64, i32, u64, i32], i32),
     "tb_swiglu_bwd": ([u64, u64, u64, u64, u64, i64, i32, i64, i64, i64, i64, i32, u64, i32], i32),
     "tb_cross_entropy": ([u64, u64, u64, u64, i32, i32, i64, i32, u64, f32, i32, u64], i32),
-    "tb_adamw_flat": ([u64, u64, i32, u64, u64, u64, i64, f32, f32, f32, f32, f32, i32, u64, u64, i32, u64], i32),
+    "tb_adamw_flat": ([u64, u64, i32, u64, u64, u64, i64, f32, f32, f32, f32, f32, i32, u64, u64, u64, i32, u64], i32),
     "tb_sqnorm_accumulate": ([u64, i32, i64, u64, f32, i32, u64], i32),
     "tb_scale_inplace": ([u64, i32, i64, u64, i32, u64], i32),
 }

@@ -95,7 +95,9 @@ class FusedAdamW(torch.optim.Optimizer):
 
     Extra (optional) state understood per step:
       * ``grad_scale``: fp32 device tensor [1] multiplied into every gradient (clip coefficient, 1/loss_scale);
-      * ``found_inf``:  fp32 device tensor [1]; non-zero skips the update on the device.
+      * ``found_inf``:  fp32 device tensor [1]; non-zero skips the update on the device.  A skipped step does not
+        advance the bias correction: the kernel counts it on the device, and ``state_dict()`` folds that count into
+        ``state["step"]`` (the only place that waits for the device).
     Parameters may carry ``_tb_lp_shard`` (bf16 tensor, same numel): the updated value is also written there.
     Gradients may be bf16 or fp32; master params and moments are fp32.
     """
@@ -105,6 +107,7 @@ class FusedAdamW(torch.optim.Optimizer):
         super().__init__(params, defaults)
         self.grad_scale: Optional[torch.Tensor] = None
         self.found_inf: Optional[torch.Tensor] = None
+        self._skipped = {}   # param -> int32 device tensor [1]: steps skipped for found_inf, not yet in state["step"]
         # flat shards of a sharding engine: switch the engine to bf16/fp32 `_tb_grad` hand-off (no fp32 .grad copies)
         engines = set()
         for group in self.param_groups:
@@ -148,13 +151,16 @@ class FusedAdamW(torch.optim.Optimizer):
                         and g.dtype in (torch.bfloat16, torch.float32)):
                     L = nat.require()
                     lp_native = lp if (lp is not None and lp.dtype == torch.bfloat16) else None   # kernel writes bf16
+                    skipped = self._skipped.get(p)
+                    if skipped is None and self.found_inf is not None:
+                        skipped = self._skipped[p] = torch.zeros(1, dtype=torch.int32, device=p.device)
                     nat.check(
                         L.tb_adamw_flat(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.bfloat16),
                                         st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(), nat.ptr(lp_native),
                                         p.numel(),
                                         group["lr"], b1, b2, group["eps"], group["weight_decay"], st["step"],
-                                        nat.ptr(self.grad_scale), nat.ptr(self.found_inf), nat.num_sms(),
-                                        nat.stream()), "tb_adamw_flat")
+                                        nat.ptr(skipped), nat.ptr(self.grad_scale), nat.ptr(self.found_inf),
+                                        nat.num_sms(), nat.stream()), "tb_adamw_flat")
                     nat.count_launch()
                     if lp is not None and lp_native is None:
                         lp.copy_(p.data.view_as(lp))           # fp16 compute copy: separate cast
@@ -165,9 +171,21 @@ class FusedAdamW(torch.optim.Optimizer):
                     unit.mark_params_updated()       # gathered copies kept across the step are stale now
         return loss
 
+    def state_dict(self):
+        """``step`` counts the updates actually applied (steps skipped for ``found_inf`` excluded), as in torch."""
+        for p, skipped in self._skipped.items():
+            self.state[p]["step"] -= int(skipped)
+            skipped.zero_()
+        return super().state_dict()
+
+    def load_state_dict(self, state_dict):
+        super().load_state_dict(state_dict)
+        self._skipped = {}
+
     def _reference_update(self, p, g, st, group, lp):
         b1, b2 = group["betas"]
         if self.found_inf is not None and float(self.found_inf) != 0.0:
+            st["step"] -= 1
             return
         g = g.float()
         if self.grad_scale is not None:
