@@ -422,8 +422,11 @@ def flash_attn_qkvpacked_tokens(qkv, num_q_heads, num_kv_heads, head_dim, batch,
     v3 = qkv.as_strided((T, hk, d), (ts, d, 1), off + (hq + hk) * d)
     backend = _pick_backend(q3, k3, v3, 0.0, None)
     if backend == "native":
-        return _FlashAttnQKVPackedFn.apply(qkv, hq, hk, d, cu_seqlens, batch, seq_len, scale, causal,
-                                           tuple(window_size))
+        # packed: the kernels launch one CTA column per sequence of cu_seqlens (the caller's batch counts rows of
+        # input_ids, e.g. 1 for a packed batch), and read cu_seqlens as int32
+        nseq = batch if cu_seqlens is None else cu_seqlens.numel() - 1
+        cu = None if cu_seqlens is None else cu_seqlens.to(torch.int32)
+        return _FlashAttnQKVPackedFn.apply(qkv, hq, hk, d, cu, nseq, seq_len, scale, causal, tuple(window_size))
     if cu_seqlens is not None:
         out = flash_attn_varlen_cu(q3, k3, v3, cu_seqlens, cu_seqlens, scale, causal, tuple(window_size))
         return out.reshape(T, hq * d)
