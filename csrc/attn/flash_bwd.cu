@@ -25,9 +25,7 @@
 #include <stdio.h>
 
 #include "../common/ptx.cuh"
-#include "../common/tensormap.h"
-#include "attn.h"
-#include "dropout.cuh"
+#include "common.cuh"
 #include "mask.cuh"
 
 namespace tb {
@@ -40,23 +38,12 @@ constexpr int kQStages = 2;
 // share the tile so that their dK / dV stay bitwise equal, so both use 64 rows.
 constexpr int bwd_q_tile(int D, bool drop) { return (D == 64 && !drop) ? 128 : 64; }
 
-struct BwdArgs {
+struct BwdArgs : AttnShape {
   const float* lse;
   const float* delta;
   uint16_t* dk;                // bf16 or fp16 (kernel template)
   uint16_t* dv;
-  const float* alibi;          // optional ALiBi slopes [Hq] (alibi_bs == 0) or [B, Hq]
-  int alibi_bs;
-  const int* cu_q;
-  const int* cu_k;
-  int B, Sq, Sk, Hq, Hk;
-  long long Tq;
   long long dk_ts, dv_ts;
-  float scale_log2, scale;
-  int causal, wl, wr;
-  int q_bs, q_off, k_bs, k_off;   // fixed-length addressing (attn.h BlockView)
-  DropoutParams drop;             // used by the kDrop instantiations only
-  long long* trace;   // optional [64 iterations][16 slots] clock64 stamps of CTA (0,0,0) (debug / profiling)
 };
 
 template <int D, bool kDrop>
@@ -94,22 +81,13 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const uint32_t lane = lane_id();
   const int b = blockIdx.z, hk = blockIdx.y, jt = blockIdx.x;
   const int group = args.Hq / args.Hk;
-  const int q_start = args.cu_q ? args.cu_q[b] : b * args.q_bs + args.q_off;
-  const int q_len = args.cu_q ? (args.cu_q[b + 1] - q_start) : args.Sq;
-  const int k_start = args.cu_k ? args.cu_k[b] : b * args.k_bs + args.k_off;
-  const int k_len = args.cu_k ? (args.cu_k[b + 1] - k_start) : args.Sk;
+  int q_start, q_len, k_start, k_len;
+  seq_bounds(args, b, q_start, q_len, k_start, k_len);
   const int n0 = jt * kTile;
   if (n0 >= k_len) return;
 
-  // query rows that can see keys [n0, n0+127]
-  const int shift = k_len - q_len;
-  int wr_eff = args.wr;
-  if (args.causal) wr_eff = (args.wr < 0) ? 0 : min(args.wr, 0);
-  const int n_last = min(n0 + kTile, k_len) - 1;
-  const int i_lo = (wr_eff < 0) ? 0 : max(0, n0 - shift - wr_eff);
-  const int i_hi = (args.wl < 0) ? (q_len - 1) : min(q_len - 1, n_last - shift + args.wl);
-  const int it_lo = i_lo / kQTile;
-  const int n_qt = (i_hi < i_lo) ? 0 : (i_hi / kQTile - it_lo + 1);
+  int it_lo, n_qt;
+  query_tile_range(n0, kTile, q_len, k_len, args.wl, args.wr, kQTile, it_lo, n_qt);
   const int n_iter = n_qt * group;
 
   if (n_iter == 0) {  // no query sees these keys: dK = dV = 0
@@ -192,7 +170,6 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   auto mma_sync = [&]() {  // named barrier of both MMA warpgroups: step (e) reads the other warpgroup's dS^T rows
     if constexpr (kDQ) asm volatile("bar.sync 3, 256;" ::: "memory"); else wg_sync();
   };
-  const bool tracing = args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
   uint32_t drop_key[2] = {0u, 0u};
   if constexpr (kDrop) {
     drop_key[0] = drop_key_part(args.drop.seed_hi, (uint32_t)(n0 + kr));
@@ -205,7 +182,6 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const int s = it % kQStages;
     const int h = iter_head(it), m0 = iter_m0(it);
     const uint32_t q_s = sQ + s * S::kQBytes, do_s = sDO + s * S::kQBytes;
-    if (tracing && it < 64) args.trace[it * 16 + 0] = clock64();
     mbar_wait(qdo_full(s), (it / kQStages) & 1);
     // ---- (a) S^T = K Q^T, (b) dP^T = V dO^T ----
     float st[kQTile / 2], dpt[kQTile / 2];
@@ -239,18 +215,10 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     wgmma_wait<0>();
     wgmma_fence_acc(st);
     wgmma_fence_acc(dpt);
-    if (tracing && it < 64) args.trace[it * 16 + 1] = clock64();
 
     // ---- P^T = exp2(S^T * scale - LSE), dS^T = P^T o (dP^T - delta) * scale ----
     const float slope_l2 = args.alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
-    // interior tile: every query row of the tile sees every key of the tile -> no per-element mask
-    bool interior = (m0 + kQTile <= q_len) && (n0 + kTile <= k_len);
-    if (interior) {
-      const int pos_first = m0 + shift, pos_last = m0 + kQTile - 1 + shift;
-      const int hi_first = (wr_eff < 0) ? (k_len - 1) : min(k_len - 1, pos_first + wr_eff);
-      const int lo_last = (args.wl < 0) ? 0 : max(0, pos_last - args.wl);
-      interior = (hi_first >= n0 + kTile - 1) && (lo_last <= n0);
-    }
+    const bool interior = tile_interior(m0, kQTile, n0, kTile, q_len, k_len, args.wl, args.wr);
     const uint32_t drop_head = kDrop ? drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)) : 0u;
     uint32_t pfrag[kQTile / 16][4], dsfrag[kQTile / 16][4];
 #pragma unroll
@@ -266,13 +234,12 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         for (int e = 0; e < 2; ++e) {
           const int qrow = m0 + c + e;
           float x = fmaf(st[4 * j + 2 * i + e], sl2, -(e ? l2.y : l2.x));
-          if (args.alibi != nullptr) x -= slope_l2 * fabsf((float)(qrow + shift - key));
+          if (args.alibi != nullptr) x -= slope_l2 * fabsf((float)(qrow + (k_len - q_len) - key));
           float pe = fast_exp2(x);
           if (!interior) {
-            const int pos = qrow + shift;
-            const int hi = (wr_eff < 0) ? (k_len - 1) : min(k_len - 1, pos + wr_eff);
-            const int lo = (args.wl < 0) ? 0 : max(0, pos - args.wl);
-            pe = (key < k_len && qrow < q_len && key >= lo && key <= hi) ? pe : 0.f;
+            int lo, hi;   // hi <= k_len - 1: keys past the sequence are invisible
+            key_bounds(qrow, q_len, k_len, args.wl, args.wr, lo, hi);
+            pe = (qrow < q_len && key >= lo && key <= hi) ? pe : 0.f;
           }
           float dpe = dpt[4 * j + 2 * i + e];
           float pv = pe;
@@ -354,7 +321,6 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
     if (tid == 0) mbar_arrive(qdo_empty(s));
-    if (tracing && it < 64) args.trace[it * 16 + 2] = clock64();
   }
   if constexpr (kDQ) {
     if (tid == 0) tma_store_wait<0>();   // staging buffers stay allocated until the reduce-adds have completed
@@ -404,22 +370,12 @@ constexpr int kDqRows = 128;   // query rows per CTA (64 per MMA warpgroup)
 constexpr int kDqKeys = 128;   // keys per K / V tile
 constexpr int kDqStages = 2;
 
-struct DqArgs {
+struct DqArgs : AttnShape {
   const float* lse;
   const float* delta;
   uint16_t* dq;                // bf16 or fp16 (kernel template)
-  const float* alibi;          // optional ALiBi slopes [Hq] (alibi_bs == 0) or [B, Hq]
-  int alibi_bs;
-  const int* cu_q;
-  const int* cu_k;
-  int B, Sq, Sk, Hq, Hk;
-  long long Tq;
   long long dq_ts;
-  float scale_log2, scale;
-  int causal, wl, wr;
   int num_q_tiles;
-  int q_bs, q_off, k_bs, k_off;   // fixed-length addressing (attn.h BlockView)
-  DropoutParams drop;             // used by the kDrop instantiations only
 };
 
 template <int D>
@@ -449,15 +405,13 @@ flash_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
   const int b = blockIdx.z, h = blockIdx.y;
   const int hk = h / (args.Hq / args.Hk);
   const int tile = args.num_q_tiles - 1 - (int)blockIdx.x;  // heavy (late) causal tiles first
-  const int q_start = args.cu_q ? args.cu_q[b] : b * args.q_bs + args.q_off;
-  const int q_len = args.cu_q ? (args.cu_q[b + 1] - q_start) : args.Sq;
-  const int k_start = args.cu_k ? args.cu_k[b] : b * args.k_bs + args.k_off;
-  const int k_len = args.cu_k ? (args.cu_k[b + 1] - k_start) : args.Sk;
+  int q_start, q_len, k_start, k_len;
+  seq_bounds(args, b, q_start, q_len, k_start, k_len);
   const int m0 = tile * kDqRows;
   if (m0 >= q_len) return;
 
   int j_lo, n_tiles;
-  key_tile_range(m0, kDqRows, q_len, k_len, args.causal, args.wl, args.wr, kDqKeys, j_lo, n_tiles);
+  key_tile_range(m0, kDqRows, q_len, k_len, args.wl, args.wr, kDqKeys, j_lo, n_tiles);
   if (n_tiles <= 0) {  // no key visible to these rows: dQ = 0
     for (int r = threadIdx.x; r < min(kDqRows, q_len - m0); r += blockDim.x) {
       uint16_t* p = args.dq + (long long)(q_start + m0 + r) * args.dq_ts + (long long)h * D;
@@ -521,7 +475,7 @@ flash_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int row = min(m0 + r0 + 8 * i, q_len - 1);
-    key_bounds(row, q_len, k_len, args.causal, args.wl, args.wr, lo[i], hi[i]);
+    key_bounds(row, q_len, k_len, args.wl, args.wr, lo[i], hi[i]);
     pos_q[i] = row + (k_len - q_len);
     if constexpr (kDrop)
       drop_row[i] = drop_row_part(drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)), (uint32_t)(m0 + r0 + 8 * i));
@@ -661,18 +615,6 @@ bwd_convert_dq_kernel(const float* __restrict__ dq_acc, uint16_t* __restrict__ d
   }
 }
 
-static long long* g_bwd_trace = nullptr;
-void flash_attn_bwd_set_trace(long long* p) { g_bwd_trace = p; }
-
-static CUtensorMap make_map_thd_b(const void* base, long long tokens, int heads, int D, long long ts, bool bf16,
-                                  int box_rows) {
-  uint64_t dims[3] = {(uint64_t)D, (uint64_t)heads, (uint64_t)tokens};
-  uint64_t strides[2] = {(uint64_t)D * 2, (uint64_t)ts * 2};
-  uint32_t box[3] = {64, 1, (uint32_t)box_rows};
-  return make_tensor_map(base, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, dims,
-                         strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
 // fp32 dQ accumulator [tokens, heads, D]: reduce-add boxes of 64 rows x 32 columns (128 bytes), 128B-swizzled
 static CUtensorMap make_map_dq_acc(float* acc, long long tokens, int heads, int D) {
   uint64_t dims[3] = {(uint64_t)D, (uint64_t)heads, (uint64_t)tokens};
@@ -714,83 +656,47 @@ static cudaError_t launch_bwd_dq(const CUtensorMap& mq, const CUtensorMap& mk, c
   return cudaGetLastError();
 }
 
-cudaError_t flash_attn_bwd(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                           const float* lse, void* dq, void* dk, void* dv, float* dq_acc, float* delta,
-                           const int* cu_q, const int* cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
-                           long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale, bool causal,
-                           int wl, int wr, long long Tq, long long Tk, long long dq_ts, long long dk_ts,
-                           long long dv_ts, int num_sms, bool is_bf16, const float* alibi_slopes,
-                           int alibi_batch_stride, cudaStream_t stream) {
-  return flash_attn_bwd_ex(q, k, v, o, dout, lse, dq, dk, dv, dq_acc, delta, cu_q, cu_k, B, Sq, Sk, Hq, Hk, D, q_ts, k_ts,
-                           v_ts, do_ts, scale, causal, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16,
-                           alibi_slopes, alibi_batch_stride, BlockView{}, 7, stream);
-}
-
-cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const void* o, const void* dout,
-                              const float* lse, void* dq, void* dk, void* dv, float* dq_acc, float* delta,
-                              const int* cu_q, const int* cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
-                              long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale, bool causal,
-                              int wl, int wr, long long Tq, long long Tk, long long dq_ts, long long dk_ts,
-                              long long dv_ts, int num_sms, bool is_bf16, const float* alibi_slopes,
-                              int alibi_batch_stride, BlockView view, int phases, cudaStream_t stream,
-                              bool deterministic) {
-  if (B == 0 || Tq == 0 || Tk == 0) return cudaSuccess;
-  if (D != 64 && D != 128) return cudaErrorInvalidValue;
-  if (Hq % Hk != 0) return cudaErrorInvalidValue;
-  const bool drop = view.p_drop > 0.f;
-  DropoutParams dp{0u, 1.f, 0u, 0u};
-  if (drop) {
-    if (view.p_drop >= 1.f) return cudaErrorInvalidValue;
-    dp.thresh24 = (uint32_t)((double)view.p_drop * 16777216.0 + 0.5);   // mirrored in dropout_keep_mask
-    dp.rp = 1.f / (1.f - view.p_drop);
-    dp.seed_lo = (uint32_t)(view.seed & 0xffffffffull);
-    dp.seed_hi = (uint32_t)(view.seed >> 32);
-  }
+cudaError_t flash_attn_bwd(const AttnParams& p, int num_sms, cudaStream_t stream) {
+  if (p.B == 0 || p.Tq == 0 || p.Tk == 0) return cudaSuccess;
+  AttnShape shape;
+  cudaError_t e = make_shape(p, shape);
+  if (e != cudaSuccess) return e;
+  const int D = p.D, Hq = p.Hq;
+  const long long Tq = p.Tq;
+  const bool is_bf16 = p.is_bf16, drop = p.p_drop > 0.f, deterministic = p.deterministic;
   // 1) delta = rowsum(dO o O), dq_acc = 0 (the deterministic path has no accumulator)
-  if (phases & 1) {
-    float* acc = deterministic ? nullptr : dq_acc;
+  if (p.phases & 1) {
+    float* acc = deterministic ? nullptr : p.dq_acc;
     const long long warps = Tq * Hq;
     const long long blocks = (warps * 32 + 255) / 256;
-#define TB_PRE(DD, BF)                                                                                       \
-  bwd_preprocess_kernel<DD, BF><<<(unsigned)blocks, 256, 0, stream>>>((const uint16_t*)o, (const uint16_t*)dout, delta, \
-                                                                      acc, Tq, Hq, do_ts)
+#define TB_PRE(DD, BF)                                                                                              \
+  bwd_preprocess_kernel<DD, BF><<<(unsigned)blocks, 256, 0, stream>>>((const uint16_t*)p.o, (const uint16_t*)p.dout, \
+                                                                      p.delta, acc, Tq, Hq, p.do_ts)
     if (D == 128) { if (is_bf16) TB_PRE(128, true); else TB_PRE(128, false); }
     else { if (is_bf16) TB_PRE(64, true); else TB_PRE(64, false); }
 #undef TB_PRE
-    cudaError_t e = cudaGetLastError();
+    e = cudaGetLastError();
     if (e != cudaSuccess) return e;
   }
   // 2) main kernel: dK / dV (+ dQ reduce-added into dq_acc unless deterministic)
-  cudaError_t e = cudaSuccess;
-  if (phases & 2) {
+  if (p.phases & 2) {
   CUtensorMap mq, mk, mv, mdo, mdq;
   try {
-    mq = make_map_thd_b(q, Tq, Hq, D, q_ts, is_bf16, bwd_q_tile(D, drop));
-    mk = make_map_thd_b(k, Tk, Hk, D, k_ts, is_bf16, kTile);
-    mv = make_map_thd_b(v, Tk, Hk, D, v_ts, is_bf16, kTile);
-    mdo = make_map_thd_b(dout, Tq, Hq, D, do_ts, is_bf16, bwd_q_tile(D, drop));
-    mdq = deterministic ? mq : make_map_dq_acc(dq_acc, Tq, Hq, D);   // unused by the deterministic kernel
+    mq = make_map_thd(p.q, Tq, Hq, D, p.q_ts, is_bf16, bwd_q_tile(D, drop));
+    mk = make_map_thd(p.k, p.Tk, p.Hk, D, p.k_ts, is_bf16, kTile);
+    mv = make_map_thd(p.v, p.Tk, p.Hk, D, p.v_ts, is_bf16, kTile);
+    mdo = make_map_thd(p.dout, Tq, Hq, D, p.do_ts, is_bf16, bwd_q_tile(D, drop));
+    mdq = deterministic ? mq : make_map_dq_acc(p.dq_acc, Tq, Hq, D);   // unused by the deterministic kernel
   } catch (const std::exception& e) {
     fprintf(stderr, "%s\n", e.what());
     return cudaErrorInvalidValue;
   }
   BwdArgs a;
-  a.lse = lse; a.delta = delta;
-  a.dk = (uint16_t*)dk; a.dv = (uint16_t*)dv;
-  a.alibi = alibi_slopes; a.alibi_bs = alibi_batch_stride;
-  a.cu_q = cu_q; a.cu_k = cu_k;
-  a.B = B; a.Sq = Sq; a.Sk = Sk; a.Hq = Hq; a.Hk = Hk;
-  a.Tq = Tq;
-  a.dk_ts = dk_ts; a.dv_ts = dv_ts;
-  a.scale = scale;
-  a.scale_log2 = scale * 1.4426950408889634f;
-  a.causal = causal ? 1 : 0;
-  a.wl = wl; a.wr = wr;
-  a.trace = g_bwd_trace;
-  a.q_bs = view.q_bs > 0 ? view.q_bs : Sq; a.q_off = view.q_off;
-  a.k_bs = view.k_bs > 0 ? view.k_bs : Sk; a.k_off = view.k_off;
-  a.drop = dp;
-  const int max_k = cu_k ? (int)Tk : Sk;
+  static_cast<AttnShape&>(a) = shape;
+  a.lse = p.lse; a.delta = p.delta;
+  a.dk = (uint16_t*)p.dk; a.dv = (uint16_t*)p.dv;
+  a.dk_ts = p.dk_ts; a.dv_ts = p.dv_ts;
+  const int max_k = p.cu_k ? (int)p.Tk : p.Sk;
   const int num_k_tiles = (max_k + kTile - 1) / kTile;
 #define TB_BWD(DD, BF, DQ)                                                                        \
   (drop ? launch_bwd<DD, BF, true, DQ>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream)         \
@@ -806,40 +712,30 @@ cudaError_t flash_attn_bwd_ex(const void* q, const void* k, const void* v, const
   if (e != cudaSuccess) return e;
   }
   // 3) dq = cast(dq_acc), or the deterministic dQ kernel
-  if ((phases & 4) && !deterministic) {
+  if ((p.phases & 4) && !deterministic) {
     const long long n = Tq * (long long)(Hq * D / 4);
     long long blocks = (n + 255) / 256;
     if (blocks > (long long)num_sms * 16) blocks = (long long)num_sms * 16;
-    if (is_bf16) bwd_convert_dq_kernel<true><<<(unsigned)blocks, 256, 0, stream>>>(dq_acc, (uint16_t*)dq, Tq, Hq * D, dq_ts);
-    else bwd_convert_dq_kernel<false><<<(unsigned)blocks, 256, 0, stream>>>(dq_acc, (uint16_t*)dq, Tq, Hq * D, dq_ts);
+    if (is_bf16) bwd_convert_dq_kernel<true><<<(unsigned)blocks, 256, 0, stream>>>(p.dq_acc, (uint16_t*)p.dq, Tq, Hq * D, p.dq_ts);
+    else bwd_convert_dq_kernel<false><<<(unsigned)blocks, 256, 0, stream>>>(p.dq_acc, (uint16_t*)p.dq, Tq, Hq * D, p.dq_ts);
     e = cudaGetLastError();
-  } else if (phases & 4) {
+  } else if (p.phases & 4) {
     CUtensorMap mq, mk, mv, mdo;
     try {
-      mq = make_map_thd_b(q, Tq, Hq, D, q_ts, is_bf16, kDqRows);
-      mk = make_map_thd_b(k, Tk, Hk, D, k_ts, is_bf16, kDqKeys);
-      mv = make_map_thd_b(v, Tk, Hk, D, v_ts, is_bf16, kDqKeys);
-      mdo = make_map_thd_b(dout, Tq, Hq, D, do_ts, is_bf16, kDqRows);
+      mq = make_map_thd(p.q, Tq, Hq, D, p.q_ts, is_bf16, kDqRows);
+      mk = make_map_thd(p.k, p.Tk, p.Hk, D, p.k_ts, is_bf16, kDqKeys);
+      mv = make_map_thd(p.v, p.Tk, p.Hk, D, p.v_ts, is_bf16, kDqKeys);
+      mdo = make_map_thd(p.dout, Tq, Hq, D, p.do_ts, is_bf16, kDqRows);
     } catch (const std::exception& e) {
       fprintf(stderr, "%s\n", e.what());
       return cudaErrorInvalidValue;
     }
     DqArgs a;
-    a.lse = lse; a.delta = delta;
-    a.dq = (uint16_t*)dq; a.dq_ts = dq_ts;
-    a.alibi = alibi_slopes; a.alibi_bs = alibi_batch_stride;
-    a.cu_q = cu_q; a.cu_k = cu_k;
-    a.B = B; a.Sq = Sq; a.Sk = Sk; a.Hq = Hq; a.Hk = Hk;
-    a.Tq = Tq;
-    a.scale = scale;
-    a.scale_log2 = scale * 1.4426950408889634f;
-    a.causal = causal ? 1 : 0;
-    a.wl = wl; a.wr = wr;
-    const int max_q = cu_q ? (int)Tq : Sq;
+    static_cast<AttnShape&>(a) = shape;
+    a.lse = p.lse; a.delta = p.delta;
+    a.dq = (uint16_t*)p.dq; a.dq_ts = p.dq_ts;
+    const int max_q = p.cu_q ? (int)Tq : p.Sq;
     a.num_q_tiles = (max_q + kDqRows - 1) / kDqRows;
-    a.q_bs = view.q_bs > 0 ? view.q_bs : Sq; a.q_off = view.q_off;
-    a.k_bs = view.k_bs > 0 ? view.k_bs : Sk; a.k_off = view.k_off;
-    a.drop = dp;
 #define TB_DQ(DD, BF)                                                           \
   (drop ? launch_bwd_dq<DD, BF, true>(mq, mk, mv, mdo, a, stream)               \
         : launch_bwd_dq<DD, BF, false>(mq, mk, mv, mdo, a, stream))

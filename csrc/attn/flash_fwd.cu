@@ -18,9 +18,7 @@
 #include <stdlib.h>
 
 #include "../common/ptx.cuh"
-#include "../common/tensormap.h"
-#include "attn.h"
-#include "dropout.cuh"
+#include "common.cuh"
 #include "mask.cuh"
 
 namespace tb {
@@ -30,28 +28,15 @@ constexpr int kBN = 128;  // keys per tile
 constexpr int kKVStages = 2;
 constexpr int kFwdThreads = 384;  // producer warpgroup + 2 MMA warpgroups
 
-struct FwdArgs {
+struct FwdArgs : AttnShape {
   uint16_t* o;                 // bf16 or fp16 (kernel template)
-  const float* alibi;          // optional ALiBi slopes [Hq] (alibi_bs == 0) or [B, Hq]
-  int alibi_bs;
   float* lse;
-  const int* cu_q;
-  const int* cu_k;
-  int B, Sq, Sk, Hq, Hk;
   long long o_ts;
-  long long Tq;
-  float scale_log2;
-  int causal, wl, wr;
   int num_q_tiles;
-  // fixed-length addressing: sequence b starts at token b * q_bs + q_off (q_bs == Sq, q_off == 0 for a dense batch);
-  // lets ring attention run on the second half of every sequence, or on half of a K/V block, without copies
-  int q_bs, q_off, k_bs, k_off;
   // blockwise (ring) attention: when non-null, the epilogue merges this block into the running fp32 accumulator
   // acc [Tq, Hq, D] / lse in place (log-sum-exp merge) and writes the merged output to o; acc_init: first block
   float* acc;
   int acc_init;
-  DropoutParams drop;   // used by the kDrop instantiations only
-  long long* trace;     // optional [64 tiles][16 slots] clock64 stamps of the first CTA (debug / profiling)
 };
 
 template <int D>
@@ -78,17 +63,15 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const int b = blockIdx.z, h = blockIdx.y;
   const int hk = h / (args.Hq / args.Hk);
   const int tile = args.num_q_tiles - 1 - (int)blockIdx.x;  // heavy (late) causal tiles first
-  const int q_start = args.cu_q ? args.cu_q[b] : b * args.q_bs + args.q_off;
-  const int q_len = args.cu_q ? (args.cu_q[b + 1] - q_start) : args.Sq;
-  const int k_start = args.cu_k ? args.cu_k[b] : b * args.k_bs + args.k_off;
-  const int k_len = args.cu_k ? (args.cu_k[b + 1] - k_start) : args.Sk;
+  int q_start, q_len, k_start, k_len;
+  seq_bounds(args, b, q_start, q_len, k_start, k_len);
   const int m0 = tile * kBM;
   if (m0 >= q_len) return;
   const bool merging = args.acc != nullptr;
 
   // KV tile range touched by this query tile
   int j_lo, n_tiles;
-  key_tile_range(m0, kBM, q_len, k_len, args.causal, args.wl, args.wr, kBN, j_lo, n_tiles);
+  key_tile_range(m0, kBM, q_len, k_len, args.wl, args.wr, kBN, j_lo, n_tiles);
 
   if (n_tiles <= 0) {  // nothing visible: O = 0, LSE = -inf (merging: the running result is unchanged)
     for (int r = threadIdx.x; r < min(kBM, q_len - m0); r += blockDim.x) {
@@ -165,14 +148,13 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   const uint32_t quad = lane & 3;
   const int r0 = wg * 64 + (warp_idx & 3) * 16 + (int)(lane >> 2);   // this thread's rows inside the tile: r0, r0 + 8
   const bool elected = (threadIdx.x & 127) == 0;
-  const bool tracing = args.trace != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 128;
   int lo[2], hi[2], pos_q[2];
   uint32_t drop_row[2] = {0u, 0u};
   float lse_prev[2] = {-INFINITY, -INFINITY};
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int row = min(m0 + r0 + 8 * i, q_len - 1);
-    key_bounds(row, q_len, k_len, args.causal, args.wl, args.wr, lo[i], hi[i]);
+    key_bounds(row, q_len, k_len, args.wl, args.wr, lo[i], hi[i]);
     pos_q[i] = row + (k_len - q_len);
     if constexpr (kDrop)
       drop_row[i] = drop_row_part(drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)), (uint32_t)(m0 + r0 + 8 * i));
@@ -193,7 +175,6 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     const int s = t % kKVStages;
     const uint32_t ph = (t / kKVStages) & 1;
     const int n0 = (j_lo + t) * kBN;
-    if (tracing && t < 64) args.trace[t * 16 + 0] = clock64();
     // ---- S = Q K^T ----
     float sacc[kBN / 2];
     mbar_wait(k_full(s), ph);
@@ -207,7 +188,6 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     wgmma_wait<0>();
     wgmma_fence_acc(sacc);
     if (elected) mbar_arrive(k_empty(s));
-    if (tracing && t < 64) args.trace[t * 16 + 1] = clock64();
 
     // ---- scale / mask / online softmax ----
     mask_score_tile<kBN>(sacc, n0, quad, lo, hi, pos_q, has_alibi, args.scale_log2, slope_l2);
@@ -315,21 +295,9 @@ flash_fwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   }
 }
 
-static long long* g_fwd_trace = nullptr;
-void flash_attn_fwd_set_trace(long long* p) { g_fwd_trace = p; }
-
-// 3-D tensor map over a token-major [tokens, heads, D] bf16 tensor with token stride `ts` elements.
-static CUtensorMap make_map_thd(const void* base, long long tokens, int heads, int D, long long ts, bool bf16) {
-  uint64_t dims[3] = {(uint64_t)D, (uint64_t)heads, (uint64_t)tokens};
-  uint64_t strides[2] = {(uint64_t)D * 2, (uint64_t)ts * 2};
-  uint32_t box[3] = {64, 1, 128};
-  return make_tensor_map(base, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, dims,
-                         strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-}
-
 template <int D, bool kBf16, bool kDrop>
 static cudaError_t launch_fwd(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv, const FwdArgs& a,
-                              int max_q_len, cudaStream_t stream) {
+                              cudaStream_t stream) {
   using S = FwdSmem<D>;
   auto kern = flash_fwd_kernel<D, kBf16, kDrop>;
   static bool configured = false;
@@ -343,68 +311,30 @@ static cudaError_t launch_fwd(const CUtensorMap& mq, const CUtensorMap& mk, cons
   return cudaGetLastError();
 }
 
-cudaError_t flash_attn_fwd(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_q,
-                           const int* cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts,
-                           long long k_ts, long long v_ts, long long o_ts, float scale, bool causal, int wl, int wr,
-                           long long Tq, long long Tk, int max_q_len, bool is_bf16, const float* alibi_slopes,
-                           int alibi_batch_stride, cudaStream_t stream) {
-  return flash_attn_fwd_ex(q, k, v, o, lse, cu_q, cu_k, B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, o_ts, scale, causal, wl,
-                           wr, Tq, Tk, max_q_len, is_bf16, alibi_slopes, alibi_batch_stride, BlockView{}, nullptr, 0,
-                           stream);
-}
-
-cudaError_t flash_attn_fwd_ex(const void* q, const void* k, const void* v, void* o, float* lse, const int* cu_q,
-                              const int* cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts,
-                              long long k_ts, long long v_ts, long long o_ts, float scale, bool causal, int wl, int wr,
-                              long long Tq, long long Tk, int max_q_len, bool is_bf16, const float* alibi_slopes,
-                              int alibi_batch_stride, BlockView view, float* acc, int acc_init,
-                              cudaStream_t stream) {
-  if (B == 0 || Tq == 0) return cudaSuccess;
-  if (D != 64 && D != 128) return cudaErrorInvalidValue;
-  if (Hq % Hk != 0) return cudaErrorInvalidValue;
+cudaError_t flash_attn_fwd(const AttnParams& p, cudaStream_t stream) {
+  if (p.B == 0 || p.Tq == 0) return cudaSuccess;
+  FwdArgs a;
+  cudaError_t e = make_shape(p, a);
+  if (e != cudaSuccess) return e;
   CUtensorMap mq, mk, mv;
   try {
-    mq = make_map_thd(q, Tq, Hq, D, q_ts, is_bf16);
-    mk = make_map_thd(k, Tk, Hk, D, k_ts, is_bf16);
-    mv = make_map_thd(v, Tk, Hk, D, v_ts, is_bf16);
+    mq = make_map_thd(p.q, p.Tq, p.Hq, p.D, p.q_ts, p.is_bf16, kBM);
+    mk = make_map_thd(p.k, p.Tk, p.Hk, p.D, p.k_ts, p.is_bf16, kBN);
+    mv = make_map_thd(p.v, p.Tk, p.Hk, p.D, p.v_ts, p.is_bf16, kBN);
   } catch (const std::exception& e) {
     fprintf(stderr, "%s\n", e.what());
     return cudaErrorInvalidValue;
   }
-  FwdArgs a;
-  a.o = (uint16_t*)o;
-  a.alibi = alibi_slopes;
-  a.alibi_bs = alibi_batch_stride;
-  a.lse = lse;
-  a.cu_q = cu_q;
-  a.cu_k = cu_k;
-  a.B = B; a.Sq = Sq; a.Sk = Sk; a.Hq = Hq; a.Hk = Hk;
-  a.o_ts = o_ts;
-  a.Tq = Tq;
-  a.scale_log2 = scale * 1.4426950408889634f;
-  a.causal = causal ? 1 : 0;
-  a.wl = wl; a.wr = wr;
-  a.trace = g_fwd_trace;
-  a.q_bs = view.q_bs > 0 ? view.q_bs : Sq; a.q_off = view.q_off;
-  a.k_bs = view.k_bs > 0 ? view.k_bs : Sk; a.k_off = view.k_off;
-  a.acc = acc; a.acc_init = acc_init;
-  const int mq_len = cu_q ? (max_q_len > 0 ? max_q_len : (int)Tq) : Sq;
-  a.num_q_tiles = (mq_len + kBM - 1) / kBM;
-  const bool drop = view.p_drop > 0.f;
-  if (drop) {
-    if (view.p_drop >= 1.f) return cudaErrorInvalidValue;
-    a.drop.thresh24 = (uint32_t)((double)view.p_drop * 16777216.0 + 0.5);   // mirrored in dropout_keep_mask
-    a.drop.rp = 1.f / (1.f - view.p_drop);
-    a.drop.seed_lo = (uint32_t)(view.seed & 0xffffffffull);
-    a.drop.seed_hi = (uint32_t)(view.seed >> 32);
-  } else {
-    a.drop = DropoutParams{0u, 1.f, 0u, 0u};
-  }
-#define TB_FWD(DD, BF)                                                                  \
-  (drop ? launch_fwd<DD, BF, true>(mq, mk, mv, a, mq_len, stream)                       \
-        : launch_fwd<DD, BF, false>(mq, mk, mv, a, mq_len, stream))
-  if (is_bf16) return (D == 128) ? TB_FWD(128, true) : TB_FWD(64, true);
-  return (D == 128) ? TB_FWD(128, false) : TB_FWD(64, false);
+  a.o = (uint16_t*)p.o;
+  a.lse = p.lse;
+  a.o_ts = p.o_ts;
+  a.num_q_tiles = ((p.cu_q ? (int)p.Tq : p.Sq) + kBM - 1) / kBM;
+  a.acc = p.acc; a.acc_init = p.acc_init;
+  const bool drop = p.p_drop > 0.f;
+#define TB_FWD(DD, BF) \
+  (drop ? launch_fwd<DD, BF, true>(mq, mk, mv, a, stream) : launch_fwd<DD, BF, false>(mq, mk, mv, a, stream))
+  if (p.is_bf16) return (p.D == 128) ? TB_FWD(128, true) : TB_FWD(64, true);
+  return (p.D == 128) ? TB_FWD(128, false) : TB_FWD(64, false);
 #undef TB_FWD
 }
 

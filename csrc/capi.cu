@@ -2,6 +2,7 @@
 // Every function returns a cudaError_t as int; pointers are raw device addresses (tensor.data_ptr()) and
 // `stream` is a cudaStream_t handle (torch.cuda.current_stream().cuda_stream).
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #include "attn/attn.h"
@@ -16,7 +17,7 @@ template <typename T>
 static inline T* P(uint64_t p) { return reinterpret_cast<T*>(p); }
 
 TB_API const char* tb_error_string(int code) { return cudaGetErrorString(static_cast<cudaError_t>(code)); }
-TB_API int tb_abi_version() { return 4; }
+TB_API int tb_abi_version() { return 5; }
 
 TB_API int tb_device_info(int device, int* num_sms, int* cc_major, int* cc_minor, long long* smem_optin) {
   cudaDeviceProp prop;
@@ -103,105 +104,28 @@ TB_API int tb_scale_inplace(uint64_t g, int is_bf16, long long n, uint64_t scale
   return (int)tb::scale_inplace(P<void>(g), is_bf16 != 0, n, P<float>(scale), num_sms, S(stream));
 }
 
-// ---- attention ----------------------------------------------------------------------------------------
-TB_API int tb_flash_attn_fwd(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t lse, uint64_t cu_q,
-                             uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts,
-                             long long k_ts, long long v_ts, long long o_ts, float scale, int causal, int wl, int wr,
-                             long long Tq, long long Tk, int max_q_len, int num_sms, uint64_t stream, int is_bf16,
-                             uint64_t alibi, int alibi_bs) {
-  (void)num_sms;
-  return (int)tb::flash_attn_fwd(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<float>(lse), P<int>(cu_q),
-                                 P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, o_ts, scale, causal != 0, wl,
-                                 wr, Tq, Tk, max_q_len, is_bf16 != 0, P<float>(alibi), alibi_bs, S(stream));
+// ---- attention (csrc/attn/attn.h) ---------------------------------------------------------------------------
+TB_API int tb_flash_attn_fwd(const tb::AttnParams* p, uint64_t stream) { return (int)tb::flash_attn_fwd(*p, S(stream)); }
+TB_API int tb_flash_attn_bwd(const tb::AttnParams* p, int num_sms, uint64_t stream) {
+  return (int)tb::flash_attn_bwd(*p, num_sms, S(stream));
 }
-TB_API int tb_flash_attn_bwd(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t dout, uint64_t lse, uint64_t dq,
-                             uint64_t dk, uint64_t dv, uint64_t dq_acc, uint64_t delta, uint64_t cu_q, uint64_t cu_k,
-                             int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts, long long k_ts,
-                             long long v_ts, long long do_ts, float scale, int causal, int wl, int wr, long long Tq,
-                             long long Tk, long long dq_ts, long long dk_ts, long long dv_ts, int num_sms,
-                             uint64_t stream, int is_bf16, uint64_t alibi, int alibi_bs) {
-  return (int)tb::flash_attn_bwd(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<void>(dout), P<float>(lse),
-                                 P<void>(dq), P<void>(dk), P<void>(dv), P<float>(dq_acc), P<float>(delta),
-                                 P<int>(cu_q), P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, do_ts, scale,
-                                 causal != 0, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16 != 0,
-                                 P<float>(alibi), alibi_bs, S(stream));
-}
-
-// Attention with dropout: the base signatures + (p_drop, seed); the mask is a pure function of (seed, head, q, k)
-// (csrc/attn/dropout.cuh), so the backward regenerates it from the same two values.
-TB_API int tb_flash_attn_fwd_dropout(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t lse, uint64_t cu_q,
-                                     uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts,
-                                     long long k_ts, long long v_ts, long long o_ts, float scale, int causal, int wl,
-                                     int wr, long long Tq, long long Tk, int max_q_len, uint64_t stream, int is_bf16,
-                                     uint64_t alibi, int alibi_bs, float p_drop, uint64_t seed) {
-  tb::BlockView view;
-  view.p_drop = p_drop; view.seed = seed;
-  return (int)tb::flash_attn_fwd_ex(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<float>(lse), P<int>(cu_q),
-                                    P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, o_ts, scale, causal != 0, wl,
-                                    wr, Tq, Tk, max_q_len, is_bf16 != 0, P<float>(alibi), alibi_bs, view, nullptr, 0,
-                                    S(stream));
-}
-TB_API int tb_flash_attn_bwd_dropout(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t dout, uint64_t lse,
-                                     uint64_t dq, uint64_t dk, uint64_t dv, uint64_t dq_acc, uint64_t delta,
-                                     uint64_t cu_q, uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
-                                     long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale,
-                                     int causal, int wl, int wr, long long Tq, long long Tk, long long dq_ts,
-                                     long long dk_ts, long long dv_ts, int num_sms, uint64_t stream, int is_bf16,
-                                     uint64_t alibi, int alibi_bs, float p_drop, uint64_t seed) {
-  tb::BlockView view;
-  view.p_drop = p_drop; view.seed = seed;
-  return (int)tb::flash_attn_bwd_ex(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<void>(dout), P<float>(lse),
-                                    P<void>(dq), P<void>(dk), P<void>(dv), P<float>(dq_acc), P<float>(delta),
-                                    P<int>(cu_q), P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, do_ts, scale,
-                                    causal != 0, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16 != 0,
-                                    P<float>(alibi), alibi_bs, view, 7, S(stream));
-}
-
-// Deterministic backward: the dropout variant's arguments (p_drop = 0: no dropout).  dK/dV come from the main kernel
-// without its dQ step, dQ from the query-stationary dQ kernel; no atomics, so repeated calls are bitwise equal.
-// dq_acc is unused.
-TB_API int tb_flash_attn_bwd_deterministic(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t dout, uint64_t lse,
-                                           uint64_t dq, uint64_t dk, uint64_t dv, uint64_t dq_acc, uint64_t delta,
-                                           uint64_t cu_q, uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
-                                           long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale,
-                                           int causal, int wl, int wr, long long Tq, long long Tk, long long dq_ts,
-                                           long long dk_ts, long long dv_ts, int num_sms, uint64_t stream, int is_bf16,
-                                           uint64_t alibi, int alibi_bs, float p_drop, uint64_t seed) {
-  tb::BlockView view;
-  view.p_drop = p_drop; view.seed = seed;
-  return (int)tb::flash_attn_bwd_ex(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<void>(dout), P<float>(lse),
-                                    P<void>(dq), P<void>(dk), P<void>(dv), P<float>(dq_acc), P<float>(delta),
-                                    P<int>(cu_q), P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, do_ts, scale,
-                                    causal != 0, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16 != 0,
-                                    P<float>(alibi), alibi_bs, view, 7, S(stream), /*deterministic=*/true);
-}
-
-// Blockwise (ring) variants: BlockView addressing + in-kernel (out, lse) merge / phased backward (csrc/attn/attn.h).
-TB_API int tb_flash_attn_block_fwd(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t lse, uint64_t cu_q,
-                                   uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D, long long q_ts,
-                                   long long k_ts, long long v_ts, long long o_ts, float scale, int causal, int wl,
-                                   int wr, long long Tq, long long Tk, uint64_t stream, int is_bf16, int q_bs, int q_off,
-                                   int k_bs, int k_off, uint64_t acc, int acc_init) {
-  tb::BlockView view;
-  view.q_bs = q_bs; view.q_off = q_off; view.k_bs = k_bs; view.k_off = k_off;
-  return (int)tb::flash_attn_fwd_ex(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<float>(lse), P<int>(cu_q),
-                                    P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, o_ts, scale, causal != 0, wl,
-                                    wr, Tq, Tk, 0, is_bf16 != 0, nullptr, 0, view, P<float>(acc), acc_init, S(stream));
-}
-TB_API int tb_flash_attn_block_bwd(uint64_t q, uint64_t k, uint64_t v, uint64_t o, uint64_t dout, uint64_t lse,
-                                   uint64_t dq, uint64_t dk, uint64_t dv, uint64_t dq_acc, uint64_t delta,
-                                   uint64_t cu_q, uint64_t cu_k, int B, int Sq, int Sk, int Hq, int Hk, int D,
-                                   long long q_ts, long long k_ts, long long v_ts, long long do_ts, float scale,
-                                   int causal, int wl, int wr, long long Tq, long long Tk, long long dq_ts,
-                                   long long dk_ts, long long dv_ts, int num_sms, uint64_t stream, int is_bf16, int q_bs,
-                                   int q_off, int k_bs, int k_off, int phases) {
-  tb::BlockView view;
-  view.q_bs = q_bs; view.q_off = q_off; view.k_bs = k_bs; view.k_off = k_off;
-  return (int)tb::flash_attn_bwd_ex(P<void>(q), P<void>(k), P<void>(v), P<void>(o), P<void>(dout), P<float>(lse),
-                                    P<void>(dq), P<void>(dk), P<void>(dv), P<float>(dq_acc), P<float>(delta),
-                                    P<int>(cu_q), P<int>(cu_k), B, Sq, Sk, Hq, Hk, D, q_ts, k_ts, v_ts, do_ts, scale,
-                                    causal != 0, wl, wr, Tq, Tk, dq_ts, dk_ts, dv_ts, num_sms, is_bf16 != 0, nullptr, 0,
-                                    view, phases, S(stream));
+// sizeof(AttnParams), then the offset of every field in declaration order, into out[0, n); returns the number of values
+TB_API int tb_attn_params_layout(long long* out, int n) {
+  using A = tb::AttnParams;
+  const long long v[] = {
+      sizeof(A),          offsetof(A, q),        offsetof(A, k),       offsetof(A, v),     offsetof(A, o),
+      offsetof(A, dout),  offsetof(A, lse),      offsetof(A, dq),      offsetof(A, dk),    offsetof(A, dv),
+      offsetof(A, dq_acc), offsetof(A, delta),   offsetof(A, q_ts),    offsetof(A, k_ts),  offsetof(A, v_ts),
+      offsetof(A, o_ts),  offsetof(A, do_ts),    offsetof(A, dq_ts),   offsetof(A, dk_ts), offsetof(A, dv_ts),
+      offsetof(A, cu_q),  offsetof(A, cu_k),     offsetof(A, B),       offsetof(A, Sq),    offsetof(A, Sk),
+      offsetof(A, Hq),    offsetof(A, Hk),       offsetof(A, D),       offsetof(A, Tq),    offsetof(A, Tk),
+      offsetof(A, scale), offsetof(A, causal),   offsetof(A, wl),      offsetof(A, wr),    offsetof(A, alibi),
+      offsetof(A, alibi_bs), offsetof(A, p_drop), offsetof(A, seed),   offsetof(A, q_bs),  offsetof(A, q_off),
+      offsetof(A, k_bs),  offsetof(A, k_off),    offsetof(A, acc),     offsetof(A, acc_init),
+      offsetof(A, phases), offsetof(A, deterministic), offsetof(A, is_bf16)};
+  const int total = (int)(sizeof(v) / sizeof(v[0]));
+  for (int i = 0; i < n && i < total; ++i) out[i] = v[i];
+  return total;
 }
 
 // ---- symmetric-memory communication ------------------------------------------------------------------------
@@ -237,14 +161,6 @@ TB_API int tb_symm_all_to_all(const uint64_t* peers, const uint64_t* pads, long 
                               int num_sms, uint64_t stream) {
   return (int)tb::symm_all_to_all(peers, pads, (size_t)src_off, P<void>(out), (size_t)chunk_bytes, rank, world, channel,
                                   epoch, P<uint32_t>(counter), num_sms, S(stream));
-}
-TB_API int tb_flash_attn_bwd_set_trace(uint64_t ptr) {
-  tb::flash_attn_bwd_set_trace(P<long long>(ptr));
-  return 0;
-}
-TB_API int tb_flash_attn_fwd_set_trace(uint64_t ptr) {
-  tb::flash_attn_fwd_set_trace(P<long long>(ptr));
-  return 0;
 }
 
 // ---- fused tensor-parallel GEMMs ---------------------------------------------------------------------------

@@ -539,6 +539,21 @@ def test_step_watchdog_dumps_stacks_of_a_hung_step(tmp_path):
     assert "fast_step" not in r.stderr                               # the healthy step left no dump
 
 
+def test_attn_params_layout_matches_the_library():
+    """The attention entry points take one ``AttnParams`` struct through ctypes, so nothing checks argument counts or
+    types: the Python mirror must have the C struct's size and every field at the C offset, in declaration order."""
+    import ctypes
+    from torchacc_b200 import _native as nat
+    from torchacc_b200.ops.attention import AttnParams
+    L = nat.lib()
+    if L is None:
+        pytest.skip("native library not built")
+    out = (nat.i64 * 64)()
+    n = L.tb_attn_params_layout(out, 64)
+    expected = [ctypes.sizeof(AttnParams)] + [getattr(AttnParams, name).offset for name, _ in AttnParams._fields_]
+    assert list(out[:n]) == expected
+
+
 def test_carry_queue_slices_jobs_by_flop_budget():
     """Host side of the carried collectives (csrc/fused/carry.cu, C++): jobs are cut into chunk ranges proportional to the
     FLOPs of the GEMM that takes them along, foreground jobs before background jobs, at most two slices per launch, every

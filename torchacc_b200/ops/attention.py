@@ -19,6 +19,7 @@ Features the native kernels do not cover (dropout > 0, ALiBi, head_dim not in {6
 """
 from __future__ import annotations
 
+import ctypes
 import math
 import os
 
@@ -62,32 +63,58 @@ def _warn_once(key, msg):
         logger.warning(msg)
 
 
+class AttnParams(ctypes.Structure):
+    """Mirror of ``AttnParams`` in csrc/attn/attn.h, field for field (``tb_attn_params_layout`` reports the C layout);
+    pointers are ``data_ptr()`` values."""
+    _fields_ = ([(n, ctypes.c_void_p) for n in ("q", "k", "v", "o", "dout", "lse", "dq", "dk", "dv", "dq_acc", "delta")]
+                + [(n, nat.i64) for n in ("q_ts", "k_ts", "v_ts", "o_ts", "do_ts", "dq_ts", "dk_ts", "dv_ts")]
+                + [("cu_q", ctypes.c_void_p), ("cu_k", ctypes.c_void_p)]
+                + [(n, nat.i32) for n in ("B", "Sq", "Sk", "Hq", "Hk", "D")] + [("Tq", nat.i64), ("Tk", nat.i64)]
+                + [("scale", nat.f32), ("causal", nat.i32), ("wl", nat.i32), ("wr", nat.i32)]
+                + [("alibi", ctypes.c_void_p), ("alibi_bs", nat.i32)]
+                + [("p_drop", nat.f32), ("seed", nat.u64)]
+                + [(n, nat.i32) for n in ("q_bs", "q_off", "k_bs", "k_off")]
+                + [("acc", ctypes.c_void_p), ("acc_init", nat.i32)]
+                + [(n, nat.i32) for n in ("phases", "deterministic", "is_bf16")])
+
+
 nat.register_signatures({
-    "tb_flash_attn_fwd": ([nat.u64] * 7 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
-                          [nat.i64, nat.i64, nat.i32, nat.i32, nat.u64, nat.i32, nat.u64, nat.i32], nat.i32),
-    "tb_flash_attn_bwd": ([nat.u64] * 13 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
-                          [nat.i64] * 5 + [nat.i32, nat.u64, nat.i32, nat.u64, nat.i32], nat.i32),
-    "tb_flash_attn_fwd_dropout": ([nat.u64] * 7 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
-                                  [nat.i64, nat.i64, nat.i32, nat.u64, nat.i32, nat.u64, nat.i32, nat.f32, nat.u64],
-                                  nat.i32),
-    "tb_flash_attn_bwd_dropout": ([nat.u64] * 13 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
-                                  [nat.i64] * 5 + [nat.i32, nat.u64, nat.i32, nat.u64, nat.i32, nat.f32, nat.u64],
-                                  nat.i32),
-    "tb_flash_attn_bwd_deterministic": ([nat.u64] * 13 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32] + [nat.i32] * 3 +
-                                        [nat.i64] * 5 + [nat.i32, nat.u64, nat.i32, nat.u64, nat.i32, nat.f32, nat.u64],
-                                        nat.i32),
+    "tb_flash_attn_fwd": ([ctypes.POINTER(AttnParams), nat.u64], nat.i32),
+    "tb_flash_attn_bwd": ([ctypes.POINTER(AttnParams), nat.i32, nat.u64], nat.i32),
+    "tb_attn_params_layout": ([ctypes.POINTER(nat.i64), nat.i32], nat.i32),
 })
+
+
+def attn_params(q3, k3, v3, o3, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, window, alibi=None, dropout=None,
+                view=(0, 0, 0, 0), grads=None, **extra) -> AttnParams:
+    """AttnParams of one call on [T, H, D] views.  ``dropout`` = (p, seed) or None; ``view`` = (q_bs, q_off, k_bs,
+    k_off); ``grads`` = (do3, dq3, dk3, dv3, dq_acc, delta) for the backward; ``extra`` sets further fields."""
+    Tq, Hq, D = q3.shape
+    ap, abs_ = _alibi_args(alibi, Hq)
+    p_drop, seed = dropout if dropout is not None else (0.0, 0)
+    p = AttnParams(q=q3.data_ptr(), k=k3.data_ptr(), v=v3.data_ptr(), o=o3.data_ptr(), lse=lse.data_ptr(),
+                   q_ts=q3.stride(0), k_ts=k3.stride(0), v_ts=v3.stride(0), o_ts=o3.stride(0),
+                   cu_q=nat.ptr(cu_q), cu_k=nat.ptr(cu_k), B=B, Sq=Sq, Sk=Sk, Hq=Hq, Hk=k3.shape[1], D=D, Tq=Tq,
+                   Tk=k3.shape[0], scale=scale, causal=int(causal), wl=window[0], wr=window[1], alibi=ap, alibi_bs=abs_,
+                   p_drop=float(p_drop), seed=int(seed), q_bs=view[0], q_off=view[1], k_bs=view[2], k_off=view[3],
+                   is_bf16=int(q3.dtype == torch.bfloat16), **{"phases": 7, **extra})
+    if grads is not None:
+        do3, dq3, dk3, dv3, dq_acc, delta = grads
+        p.dout, p.dq, p.dk, p.dv = do3.data_ptr(), dq3.data_ptr(), dk3.data_ptr(), dv3.data_ptr()
+        p.do_ts, p.dq_ts, p.dk_ts, p.dv_ts = do3.stride(0), dq3.stride(0), dk3.stride(0), dv3.stride(0)
+        p.dq_acc, p.delta = nat.ptr(dq_acc), delta.data_ptr()
+    return p
 
 
 def native_supported(q, k, v, dropout_p, alibi_slopes, pad_ok: bool = False) -> bool:
     L = nat.lib()
-    if L is None or not hasattr(L, "tb_flash_attn_fwd"):
+    if L is None:
         return False
     D = q.shape[-1]
     # head dims other than 64 / 128 are zero-padded up to the next supported size by the callers (_pad_head_dim);
     # ALiBi, fp16 and dropout (counter-based mask, csrc/attn/dropout.cuh) are native
     d_ok = D in (64, 128) or (pad_ok and D <= 128 and D % 8 == 0)
-    drop_ok = dropout_p == 0.0 or (0.0 < dropout_p < 1.0 and hasattr(L, "tb_flash_attn_fwd_dropout"))
+    drop_ok = dropout_p == 0.0 or 0.0 < dropout_p < 1.0
     return (q.is_cuda and q.dtype in (torch.bfloat16, torch.float16) and d_ok and drop_ok
             and q.stride(-1) == 1 and k.stride(-1) == 1 and v.stride(-1) == 1)
 
@@ -189,74 +216,28 @@ def _native_fwd(q3, k3, v3, cu_q, cu_k, B, Sq, Sk, scale, causal, window, alibi=
     """q3: [Tq, Hq, D] strided view (token stride arbitrary, head stride D); returns (o [Tq,Hq,D], lse [Hq,Tq]).
     ``dropout`` = (p, seed) or None."""
     Tq, Hq, D = q3.shape
-    ap, abs_ = _alibi_args(alibi, Hq)
-    Tk, Hk = k3.shape[0], k3.shape[1]
     o = torch.empty((Tq, Hq, D), dtype=q3.dtype, device=q3.device)
     lse = torch.empty((Hq, Tq), dtype=torch.float32, device=q3.device)
-    L = nat.require()
-    if dropout is not None:
-        nat.check(
-            L.tb_flash_attn_fwd_dropout(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o.data_ptr(), lse.data_ptr(),
-                                        nat.ptr(cu_q), nat.ptr(cu_k), B, Sq, Sk, Hq, Hk, D, q3.stride(0), k3.stride(0),
-                                        v3.stride(0), o.stride(0), scale, int(causal), window[0], window[1], Tq, Tk, 0,
-                                        nat.stream(), int(q3.dtype == torch.bfloat16), ap, abs_, float(dropout[0]),
-                                        int(dropout[1])), "tb_flash_attn_fwd_dropout")
-        nat.count_launch()
-        return o, lse
-    nat.check(
-        L.tb_flash_attn_fwd(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o.data_ptr(), lse.data_ptr(), nat.ptr(cu_q),
-                            nat.ptr(cu_k), B, Sq, Sk, Hq, Hk, D, q3.stride(0), k3.stride(0), v3.stride(0), o.stride(0),
-                            scale, int(causal), window[0], window[1], Tq, Tk, 0, nat.num_sms(), nat.stream(),
-                            int(q3.dtype == torch.bfloat16), ap, abs_),
-        "tb_flash_attn_fwd")
+    p = attn_params(q3, k3, v3, o, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, window, alibi, dropout)
+    nat.check(nat.require().tb_flash_attn_fwd(ctypes.byref(p), nat.stream()), "tb_flash_attn_fwd")
     nat.count_launch()
     return o, lse
 
 
 def _native_bwd(do3, q3, k3, v3, o3, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, window, dq3, dk3, dv3,
                 deterministic=False, alibi=None, dropout=None):
+    """deterministic: delta, dK/dV without the dQ step, then the query-stationary dQ kernel (no fp32 accumulator, no
+    atomics)."""
+    global DETERMINISTIC_BWD_CALLS
     Tq, Hq, D = q3.shape
-    ap, abs_ = _alibi_args(alibi, Hq)
-    Tk, Hk = k3.shape[0], k3.shape[1]
     delta = torch.empty((Hq, Tq), dtype=torch.float32, device=q3.device)
-    L = nat.require()
-    if deterministic:
-        # delta, dK/dV without the dQ step, then the query-stationary dQ kernel: no fp32 accumulator, no atomics
-        global DETERMINISTIC_BWD_CALLS
-        p, seed = dropout if dropout is not None else (0.0, 0)
-        nat.check(
-            L.tb_flash_attn_bwd_deterministic(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(),
-                                              do3.data_ptr(), lse.data_ptr(), dq3.data_ptr(), dk3.data_ptr(),
-                                              dv3.data_ptr(), 0, delta.data_ptr(), nat.ptr(cu_q), nat.ptr(cu_k), B,
-                                              Sq, Sk, Hq, Hk, D, q3.stride(0), k3.stride(0), v3.stride(0),
-                                              do3.stride(0), scale, int(causal), window[0], window[1], Tq, Tk,
-                                              dq3.stride(0), dk3.stride(0), dv3.stride(0), nat.num_sms(), nat.stream(),
-                                              int(q3.dtype == torch.bfloat16), ap, abs_, float(p), int(seed)),
-            "tb_flash_attn_bwd_deterministic")
-        nat.count_launch(3)
-        DETERMINISTIC_BWD_CALLS += 1
-        return
-    dq_acc = torch.empty((Tq, Hq, D), dtype=torch.float32, device=q3.device)
-    if dropout is not None:
-        nat.check(
-            L.tb_flash_attn_bwd_dropout(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(), do3.data_ptr(),
-                                        lse.data_ptr(), dq3.data_ptr(), dk3.data_ptr(), dv3.data_ptr(),
-                                        dq_acc.data_ptr(), delta.data_ptr(), nat.ptr(cu_q), nat.ptr(cu_k), B, Sq, Sk,
-                                        Hq, Hk, D, q3.stride(0), k3.stride(0), v3.stride(0), do3.stride(0), scale,
-                                        int(causal), window[0], window[1], Tq, Tk, dq3.stride(0), dk3.stride(0),
-                                        dv3.stride(0), nat.num_sms(), nat.stream(), int(q3.dtype == torch.bfloat16),
-                                        ap, abs_, float(dropout[0]), int(dropout[1])), "tb_flash_attn_bwd_dropout")
-        nat.count_launch(3)
-        return
-    nat.check(
-        L.tb_flash_attn_bwd(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(), do3.data_ptr(),
-                            lse.data_ptr(), dq3.data_ptr(), dk3.data_ptr(), dv3.data_ptr(), dq_acc.data_ptr(),
-                            delta.data_ptr(), nat.ptr(cu_q), nat.ptr(cu_k), B, Sq, Sk, Hq, Hk, D, q3.stride(0),
-                            k3.stride(0), v3.stride(0), do3.stride(0), scale, int(causal), window[0], window[1], Tq,
-                            Tk, dq3.stride(0), dk3.stride(0), dv3.stride(0), nat.num_sms(), nat.stream(),
-                            int(q3.dtype == torch.bfloat16), ap, abs_),
-        "tb_flash_attn_bwd")
+    dq_acc = None if deterministic else torch.empty((Tq, Hq, D), dtype=torch.float32, device=q3.device)
+    p = attn_params(q3, k3, v3, o3, lse, cu_q, cu_k, B, Sq, Sk, scale, causal, window, alibi, dropout,
+                    grads=(do3, dq3, dk3, dv3, dq_acc, delta), deterministic=int(deterministic))
+    nat.check(nat.require().tb_flash_attn_bwd(ctypes.byref(p), nat.num_sms(), nat.stream()), "tb_flash_attn_bwd")
     nat.count_launch(3)
+    if deterministic:
+        DETERMINISTIC_BWD_CALLS += 1
 
 
 class _FlashAttnFn(torch.autograd.Function):

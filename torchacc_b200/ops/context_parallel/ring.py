@@ -12,16 +12,18 @@ fp32.  Differences from the reference:
 * the causal flag is only applied to the diagonal block (the reference's lazy path passes ``causal`` to every
   block, Appendix B #5) and dq keeps the input dtype (the reference hard-codes bf16);
 * on the GPU every ring step is ONE kernel launch: the flash forward kernel merges its block into the running
-  (fp32 out, lse) pair in its epilogue (``tb_flash_attn_block_fwd``; the reference runs ~8 elementwise kernels per
-  step for the merge, utils.py:302-343), half-blocks of the zigzag layout are addressed in place (``BlockView``: no
-  ``.contiguous()`` copies), the backward runs delta / dQ-zero once, one main kernel per step that reduce-adds dQ into
-  one fp32 accumulator and writes dK/dV straight into the owner's slot, and one cast at the end;
+  (fp32 out, lse) pair in its epilogue (``tb_flash_attn_fwd`` with ``acc``; the reference runs ~8 elementwise kernels
+  per step for the merge, utils.py:302-343), half-blocks of the zigzag layout are addressed in place (sequence strides
+  and offsets of ``AttnParams``: no ``.contiguous()`` copies), the backward runs delta / dQ-zero once, one main kernel
+  per step that reduce-adds dQ into one fp32 accumulator and writes dK/dV straight into the owner's slot, and one cast
+  at the end;
 * variable-length K (``k_lens``) runs on the same kernels through ``cu_seqlens`` (valid keys packed first); nothing
   materialises an [S, S] score matrix.  With ``causal=True`` valid queries never see a padded key (keys at or before a
   valid query are valid), so ``k_lens`` only matters for non-causal attention.
 """
 from __future__ import annotations
 
+import ctypes
 import math
 from typing import List, Optional, Tuple
 
@@ -104,51 +106,26 @@ def merge_out_lse(out, lse, blk_out, blk_lse):
     return out * w_old + blk_out.float() * w_new, new_lse
 
 
-# ---- native blockwise kernels (csrc/attn: BlockView addressing, in-kernel merge, phased backward) --------------
-nat.register_signatures({
-    "tb_flash_attn_block_fwd": ([nat.u64] * 7 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32, nat.i32, nat.i32, nat.i32,
-                                nat.i64, nat.i64, nat.u64, nat.i32, nat.i32, nat.i32, nat.i32, nat.i32, nat.u64,
-                                nat.i32], nat.i32),
-    "tb_flash_attn_block_bwd": ([nat.u64] * 13 + [nat.i32] * 6 + [nat.i64] * 4 + [nat.f32, nat.i32, nat.i32, nat.i32,
-                                nat.i64, nat.i64, nat.i64, nat.i64, nat.i64, nat.i32, nat.u64, nat.i32, nat.i32,
-                                nat.i32, nat.i32, nat.i32, nat.i32], nat.i32),
-})
-
-
+# ---- native blockwise kernels (csrc/attn: strided sequence addressing, in-kernel merge, phased backward) ---------
 def native_blockwise_ok(q, k, v) -> bool:
-    L = nat.lib()
-    return (L is not None and hasattr(L, "tb_flash_attn_block_fwd") and A.native_supported(q, k, v, 0.0, None)
-            and A.get_attention_backend() in ("auto", "native") and q.shape[-1] in (64, 128))
+    return (A.native_supported(q, k, v, 0.0, None) and A.get_attention_backend() in ("auto", "native")
+            and q.shape[-1] in (64, 128))
 
 
 def _blk_fwd(q3, k3, v3, o3, lse, acc, first, B, Sq, Sk, scale, causal, window=(-1, -1), view=(0, 0, 0, 0),
              cu_k=None):
     """One ring step: attention of the addressed q rows against the addressed keys, merged into (acc, lse, o3)."""
-    Tq, Hq, D = q3.shape
-    Tk, Hk = k3.shape[0], k3.shape[1]
-    L = nat.require()
-    nat.check(
-        L.tb_flash_attn_block_fwd(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(), lse.data_ptr(), 0,
-                                  nat.ptr(cu_k), B, Sq, Sk, Hq, Hk, D, q3.stride(0), k3.stride(0), v3.stride(0),
-                                  o3.stride(0), scale, int(causal), window[0], window[1], Tq, Tk, nat.stream(),
-                                  int(q3.dtype == torch.bfloat16), view[0], view[1], view[2], view[3], acc.data_ptr(),
-                                  int(first)), "tb_flash_attn_block_fwd")
+    p = A.attn_params(q3, k3, v3, o3, lse, None, cu_k, B, Sq, Sk, scale, causal, window, view=view,
+                      acc=acc.data_ptr(), acc_init=int(first))
+    nat.check(nat.require().tb_flash_attn_fwd(ctypes.byref(p), nat.stream()), "tb_flash_attn_fwd")
     nat.count_launch()
 
 
 def _blk_bwd(do3, q3, k3, v3, o3, lse, dq3, dk3, dv3, dq_acc, delta, B, Sq, Sk, scale, causal, window, view, phases,
              cu_k=None):
-    Tq, Hq, D = q3.shape
-    Tk, Hk = k3.shape[0], k3.shape[1]
-    L = nat.require()
-    nat.check(
-        L.tb_flash_attn_block_bwd(q3.data_ptr(), k3.data_ptr(), v3.data_ptr(), o3.data_ptr(), do3.data_ptr(),
-                                  lse.data_ptr(), dq3.data_ptr(), dk3.data_ptr(), dv3.data_ptr(), dq_acc.data_ptr(),
-                                  delta.data_ptr(), 0, nat.ptr(cu_k), B, Sq, Sk, Hq, Hk, D, q3.stride(0), k3.stride(0),
-                                  v3.stride(0), do3.stride(0), scale, int(causal), window[0], window[1], Tq, Tk,
-                                  dq3.stride(0), dk3.stride(0), dv3.stride(0), nat.num_sms(), nat.stream(),
-                                  int(q3.dtype == torch.bfloat16), view[0], view[1], view[2], view[3], phases),
-        "tb_flash_attn_block_bwd")
+    p = A.attn_params(q3, k3, v3, o3, lse, None, cu_k, B, Sq, Sk, scale, causal, window, view=view,
+                      grads=(do3, dq3, dk3, dv3, dq_acc, delta), phases=phases)
+    nat.check(nat.require().tb_flash_attn_bwd(ctypes.byref(p), nat.num_sms(), nat.stream()), "tb_flash_attn_bwd")
     nat.count_launch()
 
 
