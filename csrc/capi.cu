@@ -65,6 +65,23 @@ TB_API int tb_rope_inplace(uint64_t x, uint64_t cos_t, uint64_t sin_t, uint64_t 
   return (int)tb::rope_inplace(P<void>(x), P<float>(cos_t), P<float>(sin_t), P<int>(positions), T, nheads, D,
                                token_stride, seq_len, backward != 0, num_sms, is_bf16 != 0, S(stream));
 }
+TB_API int tb_qk_norm_rope_fwd(uint64_t x, uint64_t out, uint64_t q_weight, uint64_t k_weight, uint64_t rstd,
+                               uint64_t cos_t, uint64_t sin_t, uint64_t positions, long long T, int hq, int hk, int D,
+                               long long token_stride, int seq_len, float eps, int num_sms, uint64_t stream,
+                               int is_bf16) {
+  return (int)tb::qk_norm_rope_fwd(P<void>(x), P<void>(out), P<void>(q_weight), P<void>(k_weight), P<float>(rstd),
+                                   P<float>(cos_t), P<float>(sin_t), P<int>(positions), T, hq, hk, D, token_stride,
+                                   seq_len, eps, num_sms, is_bf16 != 0, S(stream));
+}
+TB_API int tb_qk_norm_rope_bwd(uint64_t g, uint64_t x, uint64_t dx, uint64_t q_weight, uint64_t k_weight,
+                               uint64_t rstd, uint64_t dw_partial, int dw_rows, uint64_t cos_t, uint64_t sin_t,
+                               uint64_t positions, long long T, int hq, int hk, int D, long long token_stride,
+                               int seq_len, int num_sms, uint64_t stream, int is_bf16) {
+  return (int)tb::qk_norm_rope_bwd(P<void>(g), P<void>(x), P<void>(dx), P<void>(q_weight), P<void>(k_weight),
+                                   P<float>(rstd), P<float>(dw_partial), dw_rows, P<float>(cos_t), P<float>(sin_t),
+                                   P<int>(positions), T, hq, hk, D, token_stride, seq_len, num_sms, is_bf16 != 0,
+                                   S(stream));
+}
 TB_API int tb_swiglu_fwd(uint64_t g, uint64_t u, uint64_t h, long long T, int F, long long ldg, long long ldu,
                          int num_sms, uint64_t stream, int is_bf16) {
   return (int)tb::swiglu_fwd(P<void>(g), P<void>(u), P<void>(h), T, F, ldg, ldu, num_sms, is_bf16 != 0, S(stream));

@@ -1,5 +1,6 @@
 // Bandwidth-bound transformer ops for sm_90a: RMSNorm (+fused residual add) fwd/bwd, RoPE fwd/bwd (in place,
-// strided so it runs directly on the fused-QKV GEMM output), SwiGLU fwd/bwd.
+// strided so it runs directly on the fused-QKV GEMM output), per-head QK-RMSNorm + RoPE fwd/bwd (out of place on the
+// same layout), SwiGLU fwd/bwd.
 // All kernels move 16 bytes per thread per access and keep rows in registers between the reduction and the
 // normalisation pass, so each tensor is read exactly once and written exactly once.
 // Replaces the Triton liger kernels the reference patches in (reference torchacc/ops/liger.py:10-28,69-70).
@@ -290,6 +291,245 @@ cudaError_t rope_inplace(void* x, const float* cos_t, const float* sin_t, const 
   else
     rope_kernel<false><<<grid, 256, 0, stream>>>((__nv_bfloat16*)x, cos_t, sin_t, positions, T, nheads, D,
                                                   token_stride, seq_len, backward ? -1.f : 1.f);
+  return cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Per-head QK-RMSNorm + RoPE (Qwen3 q_norm / k_norm), out of place on the packed QKV layout of rope_kernel:
+//   z = x * rstd * w  (rstd = rsqrt(mean(x^2) + eps), w = q_weight or k_weight),  out = rope(z)
+// all in fp32 with one rounding at the end; V head rows are copied.  Backward, per row:
+//   u = rope^-1(g),  xhat = x * rstd,  dx = rstd * (u w - xhat * mean(u w xhat)),  dw += u * xhat.
+// A group of kQkGroup(D) lanes owns one head row: lane j holds elements [8j, 8j+8) of each half, which is exactly
+// RoPE's pairing, so the sum of squares is a shuffle reduction inside the group and the row never leaves registers.
+// Groups are a power of two wide (lanes past D/16 hold zeros); every lane of a warp runs every trip of the row loop so
+// the shuffles see full warps.  rstd is [T, Hq + Hk] fp32; the weight gradient is written as per-CTA fp32 partials
+// [gridDim.x, 2, D] (q then k), reduced in a fixed order inside the CTA: no atomics, bitwise reproducible.
+// ---------------------------------------------------------------------------------------------------
+constexpr int kQkThreads = 256;
+
+__host__ __device__ __forceinline__ int qk_group(int D) {
+  const int g = D >> 4;
+  return g <= 1 ? 1 : g <= 2 ? 2 : g <= 4 ? 4 : g <= 8 ? 8 : 16;
+}
+
+TB_DEVICE void load_cs8(const float* __restrict__ t, size_t off, float (&f)[8]) {
+  const float4* p = reinterpret_cast<const float4*>(t + off);
+  const float4 a = __ldg(p), b = __ldg(p + 1);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+}
+
+TB_DEVICE float group_sum(float v, int G) {
+  for (int o = G >> 1; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+template <bool kBf16>
+__global__ void __launch_bounds__(kQkThreads)
+qk_norm_rope_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ out,
+                        const __nv_bfloat16* __restrict__ qw, const __nv_bfloat16* __restrict__ kw,
+                        float* __restrict__ rstd_out, const float* __restrict__ cos_t,
+                        const float* __restrict__ sin_t, const int* __restrict__ positions, long long T, int hq,
+                        int hk, int D, long long ts, int seq_len, float eps) {
+  const int G = qk_group(D), half = D >> 1, lane = threadIdx.x & 31, j = lane & (G - 1);
+  const int heads = hq + 2 * hk, hqk = hq + hk;
+  const bool has_cols = j * 16 < D;
+  const long long rows = T * heads;
+  const int rows_per_warp = 32 / G;
+  const long long warp0 = (blockIdx.x * (long long)kQkThreads + threadIdx.x) >> 5;
+  const long long nwarps = ((long long)gridDim.x * kQkThreads) >> 5;
+  for (long long wr = warp0 * rows_per_warp; wr < rows; wr += nwarps * rows_per_warp) {
+    const long long row = wr + lane / G;
+    const bool live = row < rows && has_cols;
+    const long long t = row / heads;
+    const int hd = (int)(row - t * heads);
+    const long long off = t * ts + (long long)hd * D + j * 8;
+    uint4 u1 = make_uint4(0, 0, 0, 0), u2 = u1;
+    if (live) {
+      u1 = __ldcs(reinterpret_cast<const uint4*>(x + off));
+      u2 = __ldcs(reinterpret_cast<const uint4*>(x + off + half));
+    }
+    float a[8], b[8];
+    unpack8<kBf16>(u1, a);
+    unpack8<kBf16>(u2, b);
+    float ss = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) ss += a[e] * a[e] + b[e] * b[e];
+    ss = group_sum(ss, G);
+    if (!live) continue;
+    if (hd >= hqk) {   // V head: copied unchanged
+      __stcs(reinterpret_cast<uint4*>(out + off), u1);
+      __stcs(reinterpret_cast<uint4*>(out + off + half), u2);
+      continue;
+    }
+    const float rstd = rsqrtf(ss / (float)D + eps);
+    if (j == 0) rstd_out[t * hqk + hd] = rstd;
+    const __nv_bfloat16* w = hd < hq ? qw : kw;
+    float wa[8], wb[8], c[8], s[8];
+    unpack8<kBf16>(__ldg(reinterpret_cast<const uint4*>(w + j * 8)), wa);
+    unpack8<kBf16>(__ldg(reinterpret_cast<const uint4*>(w + half + j * 8)), wb);
+    const int pos = positions ? positions[t] : (int)(t % seq_len);
+    load_cs8(cos_t, (size_t)pos * half + j * 8, c);
+    load_cs8(sin_t, (size_t)pos * half + j * 8, s);
+    float o1[8], o2[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float za = a[e] * rstd * wa[e], zb = b[e] * rstd * wb[e];
+      o1[e] = za * c[e] - zb * s[e];
+      o2[e] = zb * c[e] + za * s[e];
+    }
+    __stcs(reinterpret_cast<uint4*>(out + off), pack8<kBf16>(o1));
+    __stcs(reinterpret_cast<uint4*>(out + off + half), pack8<kBf16>(o2));
+  }
+}
+
+// (two CTAs per SM: the 32 fp32 weight-gradient accumulators per thread must fit in 128 registers)
+template <bool kBf16>
+__global__ void __launch_bounds__(kQkThreads, 2)
+qk_norm_rope_bwd_kernel(const __nv_bfloat16* __restrict__ g_, const __nv_bfloat16* __restrict__ x,
+                        __nv_bfloat16* __restrict__ dx, const __nv_bfloat16* __restrict__ qw,
+                        const __nv_bfloat16* __restrict__ kw, const float* __restrict__ rstd_in,
+                        float* __restrict__ dw_partial, const float* __restrict__ cos_t,
+                        const float* __restrict__ sin_t, const int* __restrict__ positions, long long T, int hq,
+                        int hk, int D, long long ts, int seq_len) {
+  // every thread's 2 x 16 weight-gradient columns, then summed over the CTA's groups in a fixed order
+  __shared__ float red[kQkThreads][2][16];
+  const int G = qk_group(D), half = D >> 1, lane = threadIdx.x & 31, j = lane & (G - 1);
+  const int heads = hq + 2 * hk, hqk = hq + hk;
+  const bool has_cols = j * 16 < D;
+  const long long rows = T * heads;
+  const int rows_per_warp = 32 / G;
+  const long long warp0 = (blockIdx.x * (long long)kQkThreads + threadIdx.x) >> 5;
+  const long long nwarps = ((long long)gridDim.x * kQkThreads) >> 5;
+  float dq[16], dk[16];
+#pragma unroll
+  for (int e = 0; e < 16; ++e) dq[e] = dk[e] = 0.f;
+  for (long long wr = warp0 * rows_per_warp; wr < rows; wr += nwarps * rows_per_warp) {
+    const long long row = wr + lane / G;
+    const bool live = row < rows && has_cols;
+    const long long t = row / heads;
+    const int hd = (int)(row - t * heads);
+    const long long off = t * ts + (long long)hd * D + j * 8;
+    const bool norm_row = live && hd < hqk;
+    const bool is_q = hd < hq;
+    uint4 g1 = make_uint4(0, 0, 0, 0), g2 = g1, x1 = g1, x2 = g1, w1 = g1, w2 = g1;
+    float rstd = 0.f, c[8], s[8];
+    if (live) {
+      g1 = __ldcs(reinterpret_cast<const uint4*>(g_ + off));
+      g2 = __ldcs(reinterpret_cast<const uint4*>(g_ + off + half));
+    }
+    if (norm_row) {
+      x1 = __ldcs(reinterpret_cast<const uint4*>(x + off));
+      x2 = __ldcs(reinterpret_cast<const uint4*>(x + off + half));
+      const __nv_bfloat16* w = is_q ? qw : kw;
+      w1 = __ldg(reinterpret_cast<const uint4*>(w + j * 8));
+      w2 = __ldg(reinterpret_cast<const uint4*>(w + half + j * 8));
+      rstd = rstd_in[t * hqk + hd];
+      const int pos = positions ? positions[t] : (int)(t % seq_len);
+      load_cs8(cos_t, (size_t)pos * half + j * 8, c);
+      load_cs8(sin_t, (size_t)pos * half + j * 8, s);
+    } else {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) c[e] = s[e] = 0.f;
+    }
+    float ga[8], gb[8], xa[8], xb[8], wa[8], wb[8];
+    unpack8<kBf16>(g1, ga);
+    unpack8<kBf16>(g2, gb);
+    unpack8<kBf16>(x1, xa);
+    unpack8<kBf16>(x2, xb);
+    unpack8<kBf16>(w1, wa);
+    unpack8<kBf16>(w2, wb);
+    float dot = 0.f;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      const float ua = ga[e] * c[e] + gb[e] * s[e], ub = gb[e] * c[e] - ga[e] * s[e];   // rope^-1: sin -> -sin
+      xa[e] *= rstd;
+      xb[e] *= rstd;
+      ga[e] = ua;  // u, kept for dw
+      gb[e] = ub;
+      dot += ua * wa[e] * xa[e] + ub * wb[e] * xb[e];
+    }
+    dot = group_sum(dot, G) / (float)D;
+    if (!live) continue;
+    if (!norm_row) {   // V head: the gradient passes through
+      __stcs(reinterpret_cast<uint4*>(dx + off), g1);
+      __stcs(reinterpret_cast<uint4*>(dx + off + half), g2);
+      continue;
+    }
+    float o1[8], o2[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      o1[e] = rstd * (ga[e] * wa[e] - xa[e] * dot);
+      o2[e] = rstd * (gb[e] * wb[e] - xb[e] * dot);
+      if (is_q) {
+        dq[e] += ga[e] * xa[e];
+        dq[8 + e] += gb[e] * xb[e];
+      } else {
+        dk[e] += ga[e] * xa[e];
+        dk[8 + e] += gb[e] * xb[e];
+      }
+    }
+    __stcs(reinterpret_cast<uint4*>(dx + off), pack8<kBf16>(o1));
+    __stcs(reinterpret_cast<uint4*>(dx + off + half), pack8<kBf16>(o2));
+  }
+#pragma unroll
+  for (int e = 0; e < 16; ++e) {
+    red[threadIdx.x][0][e] = dq[e];
+    red[threadIdx.x][1][e] = dk[e];
+  }
+  __syncthreads();
+  // column c of weight k (0 = q, 1 = k): element c of the row lives in lane j = (c mod half) / 8 of every group, slot
+  // (c mod 8) + 8 * (c >= half); the groups are summed in thread order
+  for (int i = threadIdx.x; i < 2 * D; i += kQkThreads) {
+    const int which = i >= D, col = i - which * D;
+    const int hi = col >= half, cj = (col - hi * half) >> 3, slot = (col & 7) + 8 * hi;
+    float acc = 0.f;
+    for (int th = cj; th < kQkThreads; th += G) acc += red[th][which][slot];
+    dw_partial[(size_t)blockIdx.x * 2 * D + i] = acc;
+  }
+}
+
+static int qk_fwd_grid(long long rows, int D, int num_sms) {
+  const long long rows_per_cta = kQkThreads / qk_group(D);
+  const long long blocks = (rows + rows_per_cta - 1) / rows_per_cta;
+  return (int)(blocks < (long long)num_sms * 8 ? blocks : (long long)num_sms * 8);
+}
+
+cudaError_t qk_norm_rope_fwd(const void* x, void* out, const void* q_weight, const void* k_weight, float* rstd,
+                             const float* cos_t, const float* sin_t, const int* positions, long long T, int hq, int hk,
+                             int D, long long token_stride, int seq_len, float eps, int num_sms, bool is_bf16,
+                             cudaStream_t stream) {
+  if (T == 0) return cudaSuccess;
+  if (D % 16 != 0 || D > 256 || token_stride % 8 != 0 || hq < 0 || hk < 0) return cudaErrorInvalidValue;
+  const long long rows = T * (hq + 2 * hk);
+  if (rows == 0) return cudaSuccess;
+  const int grid = qk_fwd_grid(rows, D, num_sms);
+#define TB_ARGS                                                                                                      \
+  (const __nv_bfloat16*)x, (__nv_bfloat16*)out, (const __nv_bfloat16*)q_weight, (const __nv_bfloat16*)k_weight, rstd, \
+      cos_t, sin_t, positions, T, hq, hk, D, token_stride, seq_len, eps
+  if (is_bf16)
+    qk_norm_rope_fwd_kernel<true><<<grid, kQkThreads, 0, stream>>>(TB_ARGS);
+  else
+    qk_norm_rope_fwd_kernel<false><<<grid, kQkThreads, 0, stream>>>(TB_ARGS);
+#undef TB_ARGS
+  return cudaGetLastError();
+}
+
+cudaError_t qk_norm_rope_bwd(const void* g, const void* x, void* dx, const void* q_weight, const void* k_weight,
+                             const float* rstd, float* dw_partial, int dw_rows, const float* cos_t, const float* sin_t,
+                             const int* positions, long long T, int hq, int hk, int D, long long token_stride,
+                             int seq_len, int num_sms, bool is_bf16, cudaStream_t stream) {
+  (void)num_sms;
+  if (D % 16 != 0 || D > 256 || token_stride % 8 != 0 || hq < 0 || hk < 0) return cudaErrorInvalidValue;
+  // dw_partial is [dw_rows, 2, D] fp32: exactly dw_rows CTAs run and each writes its own row (zeros if it has no work)
+  if (dw_rows < 1 || dw_partial == nullptr) return cudaErrorInvalidValue;
+#define TB_ARGS                                                                                                   \
+  (const __nv_bfloat16*)g, (const __nv_bfloat16*)x, (__nv_bfloat16*)dx, (const __nv_bfloat16*)q_weight,          \
+      (const __nv_bfloat16*)k_weight, rstd, dw_partial, cos_t, sin_t, positions, T, hq, hk, D, token_stride, seq_len
+  if (is_bf16)
+    qk_norm_rope_bwd_kernel<true><<<dw_rows, kQkThreads, 0, stream>>>(TB_ARGS);
+  else
+    qk_norm_rope_bwd_kernel<false><<<dw_rows, kQkThreads, 0, stream>>>(TB_ARGS);
+#undef TB_ARGS
   return cudaGetLastError();
 }
 

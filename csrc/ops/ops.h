@@ -13,6 +13,16 @@ cudaError_t rmsnorm_bwd(const void* dy, const void* x, const void* w, const floa
 cudaError_t rope_inplace(void* x, const float* cos_t, const float* sin_t, const int* positions, long long T,
                          int nheads, int D, long long token_stride, int seq_len, bool backward, int num_sms,
                          bool is_bf16, cudaStream_t stream);
+// Per-head RMSNorm of the q and k rows of a packed QKV buffer followed by RoPE, out of place (V rows copied); rstd is
+// [T, hq + hk] fp32.  The backward writes dx and per-CTA weight-gradient partials dw_partial [dw_rows, 2, D] (q, k).
+cudaError_t qk_norm_rope_fwd(const void* x, void* out, const void* q_weight, const void* k_weight, float* rstd,
+                             const float* cos_t, const float* sin_t, const int* positions, long long T, int hq, int hk,
+                             int D, long long token_stride, int seq_len, float eps, int num_sms, bool is_bf16,
+                             cudaStream_t stream);
+cudaError_t qk_norm_rope_bwd(const void* g, const void* x, void* dx, const void* q_weight, const void* k_weight,
+                             const float* rstd, float* dw_partial, int dw_rows, const float* cos_t, const float* sin_t,
+                             const int* positions, long long T, int hq, int hk, int D, long long token_stride,
+                             int seq_len, int num_sms, bool is_bf16, cudaStream_t stream);
 cudaError_t swiglu_fwd(const void* g, const void* u, void* h, long long T, int F, long long ldg, long long ldu,
                        int num_sms, bool is_bf16, cudaStream_t stream);
 cudaError_t swiglu_bwd(const void* dh, const void* g, const void* u, void* dg, void* du, long long T, int F,

@@ -29,6 +29,10 @@ _SIGS = {
     "tb_rmsnorm_fwd": ([u64, u64, u64, u64, u64, u64, i32, i32, f32, i32, u64, i32], i32),
     "tb_rmsnorm_bwd": ([u64, u64, u64, u64, u64, u64, u64, i32, i32, i32, i32, u64, i32], i32),
     "tb_rope_inplace": ([u64, u64, u64, u64, i64, i32, i32, i64, i32, i32, i32, u64, i32], i32),
+    "tb_qk_norm_rope_fwd": ([u64, u64, u64, u64, u64, u64, u64, u64, i64, i32, i32, i32, i64, i32, f32, i32, u64, i32],
+                            i32),
+    "tb_qk_norm_rope_bwd": ([u64, u64, u64, u64, u64, u64, u64, i32, u64, u64, u64, i64, i32, i32, i32, i64, i32, i32,
+                             u64, i32], i32),
     "tb_swiglu_fwd": ([u64, u64, u64, i64, i32, i64, i64, i32, u64, i32], i32),
     "tb_swiglu_bwd": ([u64, u64, u64, u64, u64, i64, i32, i64, i64, i64, i64, i32, u64, i32], i32),
     "tb_cross_entropy": ([u64, u64, u64, u64, i32, i32, i64, i32, u64, f32, i32, u64], i32),

@@ -1,10 +1,12 @@
-"""Native Llama-family decoder (Llama-2/3, Qwen2-style with QKV bias) built on the sm_90a op set.
+"""Native Llama-family decoder (Llama-2/3, Qwen2-style with QKV bias, Qwen3-style with per-head q / k RMSNorm) built on
+the sm_90a op set.
 
 The reference has no model code of its own: it patches HF models (liger kernels, FA) and relies on FlashModels
 for TP/CP-aware modules (SURVEY 2.1 #27, #41, 7.1 "native Llama model definition").  This module is that native
 definition, laid out for the fused kernels:
 
-* ``qkv_proj``  : one GEMM for q|k|v, RoPE applied in place on its output, attention reads the packed buffer;
+* ``qkv_proj``  : one GEMM for q|k|v, RoPE applied in place on its output (with ``qk_norm``: the per-head q / k norm
+  and RoPE in one out-of-place kernel), attention reads the packed buffer;
 * ``gate_up_proj``: one GEMM for gate|up, SwiGLU kernel on its output;
 * RMSNorm fuses the residual add; the loss is fused linear + cross-entropy (no [T, V] logits);
 * token-major activations ``[T, H]`` throughout (T = batch * seq), so every op is a plain 2-D GEMM / row kernel.
@@ -24,7 +26,7 @@ from ..ops import attention as attn_ops
 from ..ops.cross_entropy import fused_linear_cross_entropy
 from ..ops.linear import linear
 from ..ops.rmsnorm import rmsnorm
-from ..ops.rope import rope_qkv_, rope_tables
+from ..ops.rope import qk_norm_rope_qkv, rope_qkv_, rope_tables
 from ..ops.moe import MoEMLP, load_balancing_loss
 from ..ops.swiglu import gate_up_swiglu, swiglu
 
@@ -55,6 +57,7 @@ class LlamaConfig:
     moe_intermediate_size: Optional[int] = None
     norm_topk_prob: bool = True
     router_aux_loss_coef: float = 0.0     # load-balancing loss weight, same scale as HF Mixtral's (0.02 there)
+    qk_norm: bool = False                 # Qwen3: RMSNorm of every q and k head (own [head_dim] weights) before RoPE
 
     def __post_init__(self):
         if self.head_dim is None:
@@ -79,6 +82,8 @@ class LlamaConfig:
         per = self.qkv_dim * h + h * self.num_attention_heads * self.head_dim + self._mlp_params() + 2 * h
         if self.attention_bias:
             per += self.qkv_dim
+        if self.qk_norm:
+            per += 2 * self.head_dim
         return L * per + v * h * (1 if self.tie_word_embeddings else 2) + h
 
     def flops_per_token(self, seq_len: int, causal: bool = True) -> float:
@@ -115,6 +120,30 @@ PRESETS = {
                      num_key_value_heads=2, head_dim=64, max_position_embeddings=512, num_experts=8,
                      num_experts_per_tok=2, model_type="mixtral"),
 }
+# Qwen3 / Qwen3-MoE, from the published config.json files
+_QWEN3 = dict(vocab_size=151936, head_dim=128, rope_theta=1000000.0, rms_norm_eps=1e-6, max_position_embeddings=40960,
+              qk_norm=True, model_type="qwen3")
+PRESETS.update({
+    "qwen3-0.6b": dict(_QWEN3, hidden_size=1024, intermediate_size=3072, num_hidden_layers=28, num_attention_heads=16,
+                       num_key_value_heads=8, tie_word_embeddings=True),
+    "qwen3-1.7b": dict(_QWEN3, hidden_size=2048, intermediate_size=6144, num_hidden_layers=28, num_attention_heads=16,
+                       num_key_value_heads=8, tie_word_embeddings=True),
+    "qwen3-4b": dict(_QWEN3, hidden_size=2560, intermediate_size=9728, num_hidden_layers=36, num_attention_heads=32,
+                     num_key_value_heads=8, tie_word_embeddings=True),
+    "qwen3-8b": dict(_QWEN3, hidden_size=4096, intermediate_size=12288, num_hidden_layers=36, num_attention_heads=32,
+                     num_key_value_heads=8),
+    "qwen3-30b-a3b": dict(_QWEN3, hidden_size=2048, intermediate_size=6144, moe_intermediate_size=768,
+                          num_hidden_layers=48, num_attention_heads=32, num_key_value_heads=4, num_experts=128,
+                          num_experts_per_tok=8, norm_topk_prob=True, router_aux_loss_coef=0.001,
+                          model_type="qwen3_moe"),
+    "tiny-qwen3": dict(_QWEN3, vocab_size=512, hidden_size=256, intermediate_size=512, num_hidden_layers=2,
+                       num_attention_heads=4, num_key_value_heads=2, head_dim=64, max_position_embeddings=512,
+                       tie_word_embeddings=True),
+    "tiny-qwen3-moe": dict(_QWEN3, vocab_size=512, hidden_size=256, intermediate_size=512, moe_intermediate_size=128,
+                           num_hidden_layers=2, num_attention_heads=4, num_key_value_heads=2, head_dim=64,
+                           max_position_embeddings=512, num_experts=8, num_experts_per_tok=2, norm_topk_prob=True,
+                           router_aux_loss_coef=0.001, model_type="qwen3_moe"),
+})
 
 
 def llama_config(name: str, **overrides) -> LlamaConfig:
@@ -147,6 +176,9 @@ class LlamaAttention(nn.Module):
         kw = dict(device=device, dtype=dtype)
         self.qkv_proj = nn.Linear(cfg.hidden_size, cfg.qkv_dim, bias=cfg.attention_bias, **kw)
         self.o_proj = nn.Linear(self.num_heads * self.head_dim, cfg.hidden_size, bias=False, **kw)
+        if cfg.qk_norm:
+            self.q_norm = _NormWeight(self.head_dim, cfg.rms_norm_eps, **kw)
+            self.k_norm = _NormWeight(self.head_dim, cfg.rms_norm_eps, **kw)
 
     def forward(self, x, rope, batch, seq_len, position_ids=None, cu_seqlens=None, pctx: Optional[ParallelContext] = None):
         cos, sin = rope
@@ -161,12 +193,23 @@ class LlamaAttention(nn.Module):
         window = (-1, -1)
         if self.cfg.sliding_window:
             window = (self.cfg.sliding_window - 1, 0)
+        qk_norm = None
+        if self.cfg.qk_norm:
+            wq, wk = self.q_norm.weight, self.k_norm.weight
+            if tp is not None:
+                # shared by all heads, so each rank's gradient covers only its own heads: summed over the group
+                from ..parallel.tp import tp_head_shared
+                wq, wk = tp_head_shared(wq, tp), tp_head_shared(wk, tp)
+            qk_norm = (wq, wk, self.q_norm.eps)
         if pctx is not None and pctx.cp_mesh is not None:
             from ..ops.context_parallel import cp_attention_qkvpacked
             o = cp_attention_qkvpacked(qkv, hq, hk, self.head_dim, batch, seq_len, rope, position_ids, pctx,
-                                       causal=True, window_size=window)
+                                       causal=True, window_size=window, qk_norm=qk_norm)
         else:
-            qkv = rope_qkv_(qkv, hq, hk, self.head_dim, cos, sin, position_ids, seq_len)
+            if qk_norm is not None:
+                qkv = qk_norm_rope_qkv(qkv, hq, hk, self.head_dim, *qk_norm, cos, sin, position_ids, seq_len)
+            else:
+                qkv = rope_qkv_(qkv, hq, hk, self.head_dim, cos, sin, position_ids, seq_len)
             o = attn_ops.flash_attn_qkvpacked_tokens(qkv, hq, hk, self.head_dim, batch, seq_len, causal=True,
                                                      window_size=window, cu_seqlens=cu_seqlens)
         if tp is not None:
@@ -382,15 +425,16 @@ class LlamaForCausalLM(nn.Module):
     # ---- HF interop -------------------------------------------------------------------------------------
     @torch.no_grad()
     def load_hf_state_dict(self, sd: dict, strict: bool = True):
-        """Load a HuggingFace Llama/Qwen2 state dict (separate q/k/v and gate/up projections), or a Mixtral one
-        (``mlp.gate.weight``, ``mlp.experts.gate_up_proj``, ``mlp.experts.down_proj``: the same names here)."""
+        """Load a HuggingFace Llama/Qwen2/Qwen3 state dict (separate q/k/v and gate/up projections), or a Mixtral /
+        Qwen3-MoE one (``mlp.gate.weight``, ``mlp.experts.gate_up_proj``, ``mlp.experts.down_proj``: the same names
+        here)."""
         own = {}
         L = self.config.num_hidden_layers
         g = lambda k: sd[k]
         own["model.embed_tokens.weight"] = g("model.embed_tokens.weight")
         own["model.norm.weight"] = g("model.norm.weight")
-        if not self.config.tie_word_embeddings:
-            own["lm_head.weight"] = sd.get("lm_head.weight", sd["model.embed_tokens.weight"])
+        # tied: lm_head.weight is the embedding parameter, listed under both names by state_dict()
+        own["lm_head.weight"] = sd.get("lm_head.weight", sd["model.embed_tokens.weight"])
         for i in range(L):
             p = f"model.layers.{i}."
             own[p + "input_layernorm.weight"] = g(p + "input_layernorm.weight")
@@ -401,6 +445,9 @@ class LlamaForCausalLM(nn.Module):
                 own[p + "self_attn.qkv_proj.bias"] = torch.cat(
                     [g(p + "self_attn.q_proj.bias"), g(p + "self_attn.k_proj.bias"), g(p + "self_attn.v_proj.bias")], 0)
             own[p + "self_attn.o_proj.weight"] = g(p + "self_attn.o_proj.weight")
+            if self.config.qk_norm:
+                own[p + "self_attn.q_norm.weight"] = g(p + "self_attn.q_norm.weight")
+                own[p + "self_attn.k_norm.weight"] = g(p + "self_attn.k_norm.weight")
             if self.config.num_experts:
                 for name in ("mlp.gate.weight", "mlp.experts.gate_up_proj", "mlp.experts.down_proj"):
                     own[p + name] = g(p + name)

@@ -7,11 +7,11 @@ from .cross_entropy import cross_entropy, fused_linear_cross_entropy
 from .linear import Linear, gemm, linear
 from .liger import (apply_liger_kernel, apply_liger_kernel_to_llama, apply_liger_kernel_to_mixtral,
                     apply_liger_kernel_to_olmoe, apply_liger_kernel_to_qwen2, apply_liger_kernel_to_qwen2_moe,
-                    apply_liger_kernel_to_qwen3_moe)
+                    apply_liger_kernel_to_qwen3, apply_liger_kernel_to_qwen3_moe)
 from .moe import MoEMLP, moe_experts, moe_router
 from .optim import FusedAdamW, grad_sqnorm
 from .rmsnorm import RMSNorm, rmsnorm
-from .rope import apply_rope, rope_qkv_, rope_tables
+from .rope import apply_rope, qk_norm_rope_qkv, rope_qkv_, rope_tables
 from .sdpa import scaled_dot_product_attention
 from .swiglu import swiglu
 from . import context_parallel

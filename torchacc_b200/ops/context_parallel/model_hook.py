@@ -3,7 +3,7 @@ from __future__ import annotations
 
 import torch
 
-from ..rope import rope_qkv_
+from ..rope import qk_norm_rope_qkv, rope_qkv_
 from .comm import _rank, _world
 from .ring import ring_attention, zigzag_positions, zigzag_split
 from .two_d import context_parallel_2d
@@ -39,11 +39,19 @@ def cp_local_positions(batch: int, seq_local: int, pctx, device) -> torch.Tensor
 
 
 def cp_attention_qkvpacked(qkv, hq, hk, d, batch, seq_local, rope, position_ids, pctx, causal=True,
-                           window_size=(-1, -1)):
-    """qkv: [batch*seq_local, (hq+2hk)*d] token-major local shard -> [batch*seq_local, hq*d]."""
+                           window_size=(-1, -1), qk_norm=None):
+    """qkv: [batch*seq_local, (hq+2hk)*d] token-major local shard -> [batch*seq_local, hq*d].  ``qk_norm``:
+    ``(q_weight, k_weight, eps)`` of a per-head q / k RMSNorm applied before RoPE (per token and head, so it commutes
+    with the all-to-all)."""
     mesh, mode, zig = _layout(pctx)
     cos, sin = rope
     T = qkv.shape[0]
+
+    def rope_(x, hq_, hk_, pos, seq):
+        if qk_norm is not None:
+            return qk_norm_rope_qkv(x, hq_, hk_, d, *qk_norm, cos, sin, pos, seq)
+        return rope_qkv_(x, hq_, hk_, d, cos, sin, pos, seq)
+
     if mode == "ulysses":
         cp = mesh.get_sp_num()
         S = seq_local * cp
@@ -57,7 +65,7 @@ def cp_attention_qkvpacked(qkv, hq, hk, d, batch, seq_local, rope, position_ids,
             hk_ = k_.shape[2]
             packed = torch.cat([q_.reshape(B_ * S_, hq_ * d), k_.reshape(B_ * S_, hk_ * d),
                                 v_.reshape(B_ * S_, hk_ * d)], 1).contiguous()
-            packed = rope_qkv_(packed, hq_, hk_, d, cos, sin, None, S_)
+            packed = rope_(packed, hq_, hk_, None, S_)
             q2 = packed[:, :hq_ * d].reshape(B_, S_, hq_, d)
             k2 = packed[:, hq_ * d:(hq_ + hk_) * d].reshape(B_, S_, hk_, d)
             v2 = packed[:, (hq_ + hk_) * d:].reshape(B_, S_, hk_, d)
@@ -68,7 +76,7 @@ def cp_attention_qkvpacked(qkv, hq, hk, d, batch, seq_local, rope, position_ids,
         return out.reshape(T, hq * d)
     # ring / 2d: RoPE on the local tokens with their global positions, then blockwise attention
     pos = position_ids if position_ids is not None else cp_local_positions(batch, seq_local, pctx, qkv.device)
-    qkv = rope_qkv_(qkv, hq, hk, d, cos, sin, pos, seq_local)
+    qkv = rope_(qkv, hq, hk, pos, seq_local)
     q = qkv[:, :hq * d].reshape(batch, seq_local, hq, d)
     k = qkv[:, hq * d:(hq + hk) * d].reshape(batch, seq_local, hk, d)
     v = qkv[:, (hq + hk) * d:].reshape(batch, seq_local, hk, d)

@@ -162,6 +162,16 @@ def apply_liger_kernel_to_qwen2(rope: bool = True, cross_entropy: bool = False, 
         _patch_rope(modeling_qwen2)
 
 
+def apply_liger_kernel_to_qwen3(rope: bool = True, cross_entropy: bool = False, fused_linear_cross_entropy: bool = True,
+                                rms_norm: bool = True, swiglu: bool = True, model: Optional[nn.Module] = None) -> None:
+    """Dense Qwen3.  Its per-head ``q_norm`` / ``k_norm`` are ``Qwen3RMSNorm`` modules on contiguous [B, S, H, D]
+    views, so the RMSNorm class patch puts them on the native kernel too."""
+    from transformers.models.qwen3 import modeling_qwen3
+    _patch_family(modeling_qwen3, "Qwen3", rms_norm, swiglu, fused_linear_cross_entropy)
+    if rope:
+        _patch_rope(modeling_qwen3)
+
+
 def experts_forward(self, hidden_states, top_k_index, top_k_weights):
     """HF 3-D experts module (``gate_up_proj [E, 2F, H]``, ``down_proj [E, H, F]``) on the grouped GEMM + routing
     kernels (ops/moe.py).  HF's router and its auxiliary loss stay HF's."""
@@ -249,6 +259,7 @@ def apply_liger_kernel(model: Optional[nn.Module] = None) -> None:
     if transformers is not None:
         families = {"transformers.models.llama.": apply_liger_kernel_to_llama,
                     "transformers.models.qwen2.": apply_liger_kernel_to_qwen2,
+                    "transformers.models.qwen3.": apply_liger_kernel_to_qwen3,
                     "transformers.models.mixtral.": apply_liger_kernel_to_mixtral,
                     "transformers.models.qwen2_moe.": apply_liger_kernel_to_qwen2_moe,
                     "transformers.models.qwen3_moe.": apply_liger_kernel_to_qwen3_moe,

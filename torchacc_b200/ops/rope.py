@@ -167,3 +167,85 @@ def rope_qkv_(qkv: torch.Tensor, num_q_heads: int, num_kv_heads: int, head_dim: 
     if positions is not None and positions.dtype != torch.int32:
         positions = positions.to(torch.int32)
     return _RopeQKVFn.apply(qkv, num_q_heads, num_kv_heads, head_dim, cos, sin, positions, seq_len)
+
+
+class _QKNormRopeQKVFn(torch.autograd.Function):
+    """Per-head RMSNorm (own weight for q and for k) then RoPE on a fused QKV buffer, out of place, one kernel each way.
+    The pre-norm input and the per-row rstd are saved; the weight gradients come from fp32 per-CTA partials summed
+    here (no atomics)."""
+
+    @staticmethod
+    def forward(ctx, qkv, q_weight, k_weight, hq, hk, d, eps, cos, sin, positions, seq_len):
+        T = qkv.shape[0]
+        out = torch.empty_like(qkv)
+        rstd = torch.empty((T, hq + hk), dtype=torch.float32, device=qkv.device)
+        L = nat.require()
+        nat.check(
+            L.tb_qk_norm_rope_fwd(qkv.data_ptr(), out.data_ptr(), q_weight.data_ptr(), k_weight.data_ptr(),
+                                  rstd.data_ptr(), cos.data_ptr(), sin.data_ptr(), nat.ptr(positions), T, hq, hk, d,
+                                  qkv.stride(0), seq_len, eps, nat.num_sms(), nat.stream(), nat.bf16_flag(qkv)),
+            "tb_qk_norm_rope_fwd")
+        nat.count_launch()
+        ctx.cfg = (hq, hk, d, seq_len)
+        ctx.save_for_backward(qkv, q_weight, k_weight, rstd, cos, sin, positions)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        hq, hk, d, seq_len = ctx.cfg
+        qkv, q_weight, k_weight, rstd, cos, sin, positions = ctx.saved_tensors
+        T = qkv.shape[0]
+        g = g.contiguous()
+        dqkv = torch.empty_like(qkv)
+        # one fp32 [2, d] partial per CTA (q, k); two resident CTAs per SM, fewer when there are fewer rows of heads
+        rows_per_cta = 256 // _qk_group(d)
+        parts = max(1, min(nat.num_sms() * 2, -(-T * (hq + 2 * hk) // rows_per_cta)))
+        dw_part = torch.empty((parts, 2, d), dtype=torch.float32, device=qkv.device)
+        L = nat.require()
+        nat.check(
+            L.tb_qk_norm_rope_bwd(g.data_ptr(), qkv.data_ptr(), dqkv.data_ptr(), q_weight.data_ptr(),
+                                  k_weight.data_ptr(), rstd.data_ptr(), dw_part.data_ptr(), parts, cos.data_ptr(),
+                                  sin.data_ptr(), nat.ptr(positions), T, hq, hk, d, qkv.stride(0), seq_len,
+                                  nat.num_sms(), nat.stream(), nat.bf16_flag(qkv)),
+            "tb_qk_norm_rope_bwd")
+        nat.count_launch()
+        dw = dw_part.sum(0)
+        return (dqkv, dw[0].to(q_weight.dtype), dw[1].to(k_weight.dtype), None, None, None, None, None, None, None,
+                None)
+
+
+def _qk_group(d: int) -> int:
+    """Lanes per head row in the fused kernel: d / 16 rounded up to a power of two."""
+    g = 1
+    while g < d // 16:
+        g *= 2
+    return g
+
+
+def _qk_norm_rope_ref(qkv, hq, hk, d, q_weight, k_weight, eps, cos, sin, positions, seq_len):
+    from .rmsnorm import rmsnorm_ref
+    T = qkv.shape[0]
+    pos = positions if positions is not None else torch.arange(T, device=qkv.device) % seq_len
+    q = rmsnorm_ref(qkv[:, :hq * d].reshape(T, hq, d), q_weight, eps)[0]
+    k = rmsnorm_ref(qkv[:, hq * d:(hq + hk) * d].reshape(T, hk, d), k_weight, eps)[0]
+    q, k = _rope_ref(q, cos, sin, pos, 1.0), _rope_ref(k, cos, sin, pos, 1.0)
+    return torch.cat([q.reshape(T, hq * d), k.reshape(T, hk * d), qkv[:, (hq + hk) * d:]], 1)
+
+
+def qk_norm_rope_qkv(qkv: torch.Tensor, num_q_heads: int, num_kv_heads: int, head_dim: int, q_weight: torch.Tensor,
+                     k_weight: torch.Tensor, eps: float, cos: torch.Tensor, sin: torch.Tensor,
+                     positions: Optional[torch.Tensor] = None, seq_len: Optional[int] = None) -> torch.Tensor:
+    """Qwen3's per-head q / k RMSNorm followed by RoPE on a fused QKV activation ``[T, (Hq + 2 Hk) D]`` (q | k | v along
+    the last dim).  Returns a new tensor: q and k rows are normalised with ``q_weight`` / ``k_weight`` ([D] each) and
+    rotated, V is copied.  The norm and the rotation run in fp32 with one rounding at the end."""
+    if seq_len is None:
+        seq_len = cos.shape[0]
+    if positions is not None and positions.dtype != torch.int32:
+        positions = positions.to(torch.int32)
+    if nat.use_native(qkv, q_weight, k_weight) and nat.is_half(qkv, q_weight, k_weight) and head_dim % 16 == 0 \
+            and head_dim <= 256 and qkv.dim() == 2 and qkv.shape[1] == (num_q_heads + 2 * num_kv_heads) * head_dim:
+        qkv = qkv.contiguous()
+        return _QKNormRopeQKVFn.apply(qkv, q_weight.contiguous(), k_weight.contiguous(), num_q_heads, num_kv_heads,
+                                      head_dim, eps, cos, sin, positions, seq_len)
+    return _qk_norm_rope_ref(qkv, num_q_heads, num_kv_heads, head_dim, q_weight, k_weight, eps, cos, sin, positions,
+                             seq_len)

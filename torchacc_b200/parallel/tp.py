@@ -222,6 +222,12 @@ def tp_replicated(p, tp: TPContext):
     return _ReplicatedParam.apply(p, tp) if (tp is not None and tp.sequence_parallel) else p
 
 
+def tp_head_shared(p, tp: TPContext):
+    """A parameter applied to every attention head (Qwen3's q / k norm weights): each rank holds it in full but only
+    sees its own heads, so its gradient is summed over the group with or without sequence parallelism."""
+    return _ReplicatedParam.apply(p, tp) if tp is not None else p
+
+
 def gather_tokens(x, tp: TPContext):
     return _GatherTokens.apply(x, tp)
 
