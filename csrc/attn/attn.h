@@ -48,5 +48,9 @@ struct AttnParams {
 
 cudaError_t flash_attn_fwd(const AttnParams& p, cudaStream_t stream);
 cudaError_t flash_attn_bwd(const AttnParams& p, int num_sms, cudaStream_t stream);
+// Phase profile of the head-dim-64 bf16 backward main kernel (benchmarks/attn_bwd_phases.py): while buf is set, that
+// kernel runs an instrumented build that writes clock64() stamps of key tiles [0, ctas) of kv head 0, sequence 0 into
+// buf (ctas records; layout in flash_bwd.cu at kProfHead).  Null turns it off.  Returns the u64 words per record.
+long long attn_bwd_set_profile(unsigned long long* buf, long long ctas);
 
 }  // namespace tb

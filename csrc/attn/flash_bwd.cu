@@ -24,6 +24,8 @@
 #include <math.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../common/ptx.cuh"
 #include "common.cuh"
 #include "mask.cuh"
@@ -38,13 +40,36 @@ constexpr int kQStages = 2;
 // share the tile so that their dK / dV stay bitwise equal, so both use 64 rows.
 constexpr int bwd_q_tile(int D, bool drop) { return (D == 64 && !drop) ? 128 : 64; }
 
+// Phase profile of the main kernel (kProf instantiations, attn_bwd_set_profile): for the CTAs of kv head 0, sequence
+// 0 and key tiles [0, prof_ctas), one elected thread per role writes clock64() stamps into a record of kProfCtaWords
+// u64 at prof + blockIdx.x * kProfCtaWords:
+//   [0] n_iter  [1] %smid  [2] CTA start  [3] K/V landed  [4] / [5] MMA warpgroup 0 / 1 done  [6] producer done
+//   [kProfHead + it * kProfSlots + ...] for iterations it < kProfIters:
+//     [0, kProfWgSlots) warpgroup 0 phase ends, [kProfWgSlots, 2 kProfWgSlots) warpgroup 1, then the producer's
+//     empty-wait done and stage issued.  Phase order: benchmarks/attn_bwd_phases.py.
+constexpr int kProfHead = 8, kProfWgSlots = 10, kProfSlots = 2 * kProfWgSlots + 2, kProfIters = 256;
+constexpr long long kProfCtaWords = kProfHead + (long long)kProfIters * kProfSlots;
+
 struct BwdArgs : AttnShape {
   const float* lse;
   const float* delta;
   uint16_t* dk;                // bf16 or fp16 (kernel template)
   uint16_t* dv;
   long long dk_ts, dv_ts;
+  unsigned long long* prof;    // kProf only
+  long long prof_ctas;
 };
+
+__device__ __forceinline__ unsigned long long prof_clock() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%clock64;" : "=l"(t)::"memory");
+  return t;
+}
+__device__ __forceinline__ unsigned long long smid() {
+  uint32_t s;
+  asm volatile("mov.u32 %0, %%smid;" : "=r"(s));
+  return s;
+}
 
 template <int D, bool kDrop>
 struct BwdSmem {
@@ -67,7 +92,8 @@ struct BwdSmem {
 
 // kDQ = false drops step (e) -- the dS^T stores, the dQ MMA and the reduce-adds -- and leaves dK / dV only; the
 // deterministic backward computes dQ afterwards in flash_bwd_dq_kernel.
-template <int D, bool kBf16, bool kDrop, bool kDQ>
+// kProf = true adds the phase stamps described at kProfHead.
+template <int D, bool kBf16, bool kDrop, bool kDQ, bool kProf = false>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                  const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
@@ -77,6 +103,8 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   constexpr int kQTile = S::kQTile;
   constexpr int kQChunk = kQTile * 128;   // bytes of one 64-column chunk of a Q / dO stage
 
+  unsigned long long t_start = 0;
+  if constexpr (kProf) t_start = prof_clock();
   const int warp_idx = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
   const uint32_t lane = lane_id();
   const int b = blockIdx.z, hk = blockIdx.y, jt = blockIdx.x;
@@ -120,6 +148,23 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
   }
   __syncthreads();
 
+  // this CTA's phase record, or null
+  unsigned long long* prof = nullptr;
+  if constexpr (kProf) {
+    if (b == 0 && hk == 0 && jt < args.prof_ctas) prof = args.prof + (long long)jt * kProfCtaWords;
+    if (prof != nullptr && threadIdx.x == 0) {
+      prof[0] = (unsigned long long)n_iter;
+      prof[1] = smid();
+      prof[2] = t_start;
+    }
+  }
+  // stamp slot `slot` of iteration `it` (one elected thread per role calls it)
+  auto stamp = [&](int it, int slot) {
+    if constexpr (kProf) {
+      if (prof != nullptr && it < kProfIters) prof[kProfHead + it * kProfSlots + slot] = prof_clock();
+    }
+  };
+
   // iteration -> (q head, q tile): heads outer, tiles inner
   auto iter_head = [&](int it) { return hk * group + it / n_qt; };
   auto iter_m0 = [&](int it) { return (it_lo + it % n_qt) * kQTile; };
@@ -137,6 +182,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       for (int it = 0; it < n_iter; ++it) {
         const int s = it % kQStages;
         mbar_wait(qdo_empty(s), ((it / kQStages) & 1) ^ 1);
+        stamp(it, 2 * kProfWgSlots);
         mbar_arrive_expect_tx(qdo_full(s), 2 * S::kQBytes);
         const int h = iter_head(it), row0 = q_start + iter_m0(it);
 #pragma unroll
@@ -144,6 +190,10 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           tma_load_3d(sQ + s * S::kQBytes + c * kQChunk, &tmap_q, qdo_full(s), c * 64, h, row0);
           tma_load_3d(sDO + s * S::kQBytes + c * kQChunk, &tmap_do, qdo_full(s), c * 64, h, row0);
         }
+        stamp(it, 2 * kProfWgSlots + 1);
+      }
+      if constexpr (kProf) {
+        if (prof != nullptr) prof[6] = prof_clock();
       }
     }
     return;
@@ -176,13 +226,20 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     drop_key[1] = drop_key_part(args.drop.seed_hi, (uint32_t)(n0 + kr + 8));
   }
 
+  const int wslot = wg * kProfWgSlots;
+  auto mark = [&](int it, int slot) { if (tid == 0) stamp(it, wslot + slot); };   // phase ends of this warpgroup
+
   float dv[D / 2], dk[D / 2];
   mbar_wait(kv_full, 0);
+  if constexpr (kProf) {
+    if (prof != nullptr && threadIdx.x == 128) prof[3] = prof_clock();
+  }
   for (int it = 0; it < n_iter; ++it) {
     const int s = it % kQStages;
     const int h = iter_head(it), m0 = iter_m0(it);
     const uint32_t q_s = sQ + s * S::kQBytes, do_s = sDO + s * S::kQBytes;
     mbar_wait(qdo_full(s), (it / kQStages) & 1);
+    mark(it, 0);
     // ---- (a) S^T = K Q^T, (b) dP^T = V dO^T ----
     float st[kQTile / 2], dpt[kQTile / 2];
     wgmma_fence_acc(st);
@@ -197,6 +254,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
       wgmma_ss<kQTile, kBf16, 0, 0>(dpt, desc_kmajor_sw128(sV_w + (kk / 4) * 16384, kk % 4),
                                     desc_kmajor_sw128(do_s + (kk / 4) * kQChunk, kk % 4), kk != 0);
     wgmma_commit();
+    mark(it, 1);
     // row statistics of this query tile, loaded while the MMAs run (the previous tile's readers are past their dS^T
     // barrier)
 #pragma unroll
@@ -211,66 +269,79 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         stat[r] = ok ? args.delta[off] : 0.f;
       }
     }
+    mark(it, 2);
     mma_sync();           // statistics visible; every reader of the previous dS^T tile is done with it
+    mark(it, 3);
     wgmma_wait<0>();
     wgmma_fence_acc(st);
     wgmma_fence_acc(dpt);
+    mark(it, 4);
 
     // ---- P^T = exp2(S^T * scale - LSE), dS^T = P^T o (dP^T - delta) * scale ----
     const float slope_l2 = args.alibi ? args.alibi[(long long)b * args.alibi_bs + h] * 1.4426950408889634f : 0.f;
     const bool interior = tile_interior(m0, kQTile, n0, kTile, q_len, k_len, args.wl, args.wr);
     const uint32_t drop_head = kDrop ? drop_head_part(args.drop.seed_lo, (uint32_t)(b * args.Hq + h)) : 0u;
     uint32_t pfrag[kQTile / 16][4], dsfrag[kQTile / 16][4];
+    // kMasked = false: an interior tile without ALiBi, where P^T is exp2 alone.  The test is uniform over the tile, so
+    // it is taken once here: folded into the loop, the compiler predicates the mask and ALiBi arithmetic and every
+    // element pays for it.
+    auto softmax_bwd = [&](auto masked) {
+      constexpr bool kMasked = decltype(masked)::value;
 #pragma unroll
-    for (int j = 0; j < kQTile / 8; ++j) {
-      const int c = 8 * j + 2 * (int)quad;                 // query columns c, c + 1 of the tile
-      const float2 l2 = *reinterpret_cast<const float2*>(stat + c);
-      const float2 dl = *reinterpret_cast<const float2*>(stat + kQTile + c);
+      for (int j = 0; j < kQTile / 8; ++j) {
+        const int c = 8 * j + 2 * (int)quad;                 // query columns c, c + 1 of the tile
+        const float2 l2 = *reinterpret_cast<const float2*>(stat + c);
+        const float2 dl = *reinterpret_cast<const float2*>(stat + kQTile + c);
 #pragma unroll
-      for (int i = 0; i < 2; ++i) {                        // key rows kr, kr + 8
-        const int key = n0 + kr + 8 * i;
-        float p[2], ds[2];
+        for (int i = 0; i < 2; ++i) {                        // key rows kr, kr + 8
+          const int key = n0 + kr + 8 * i;
+          float p[2], ds[2];
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int qrow = m0 + c + e;
-          float x = fmaf(st[4 * j + 2 * i + e], sl2, -(e ? l2.y : l2.x));
-          if (args.alibi != nullptr) x -= slope_l2 * fabsf((float)(qrow + (k_len - q_len) - key));
-          float pe = fast_exp2(x);
-          if (!interior) {
-            int lo, hi;   // hi <= k_len - 1: keys past the sequence are invisible
-            key_bounds(qrow, q_len, k_len, args.wl, args.wr, lo, hi);
-            pe = (qrow < q_len && key >= lo && key <= hi) ? pe : 0.f;
+          for (int e = 0; e < 2; ++e) {
+            const int qrow = m0 + c + e;
+            float x = fmaf(st[4 * j + 2 * i + e], sl2, -(e ? l2.y : l2.x));
+            if (kMasked && args.alibi != nullptr) x -= slope_l2 * fabsf((float)(qrow + (k_len - q_len) - key));
+            float pe = fast_exp2(x);
+            if (kMasked && !interior) {
+              int lo, hi;   // hi <= k_len - 1: keys past the sequence are invisible
+              key_bounds(qrow, q_len, k_len, args.wl, args.wr, lo, hi);
+              pe = (qrow < q_len && key >= lo && key <= hi) ? pe : 0.f;
+            }
+            float dpe = dpt[4 * j + 2 * i + e];
+            float pv = pe;
+            if constexpr (kDrop) {
+              // dV += (P o mask / (1-p))^T dO; d(dropped P) -> dP: the same mask and 1/(1-p)
+              const bool keep = drop_keep(drop_row_part(drop_head, (uint32_t)qrow), drop_key[i], args.drop.thresh24);
+              pv = keep ? pe * args.drop.rp : 0.f;
+              dpe = keep ? dpe * args.drop.rp : 0.f;
+            }
+            p[e] = pv;
+            ds[e] = pe * (dpe - (e ? dl.y : dl.x)) * sc;
           }
-          float dpe = dpt[4 * j + 2 * i + e];
-          float pv = pe;
-          if constexpr (kDrop) {
-            // dV += (P o mask / (1-p))^T dO; d(dropped P) -> dP: the same mask and 1/(1-p)
-            const bool keep = drop_keep(drop_row_part(drop_head, (uint32_t)qrow), drop_key[i], args.drop.thresh24);
-            pv = keep ? pe * args.drop.rp : 0.f;
-            dpe = keep ? dpe * args.drop.rp : 0.f;
+          pfrag[j >> 1][(j & 1) * 2 + i] = pack_h2<kBf16>(p[0], p[1]);
+          const uint32_t dsp = pack_h2<kBf16>(ds[0], ds[1]);
+          dsfrag[j >> 1][(j & 1) * 2 + i] = dsp;
+          if constexpr (kDQ) {
+            // dS^T -> smem row (key) of chunk j / 8, 128B-swizzled: 16-byte unit u of row r lives at unit (u ^ (r & 7))
+            const uint32_t r = (uint32_t)(kr + 8 * i), u = (uint32_t)j & 7u;
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(sDS + (j >> 3) * 16384 + r * 128u + ((u ^ (r & 7u)) << 4) +
+                                                            4u * quad),
+                         "r"(dsp)
+                         : "memory");
           }
-          p[e] = pv;
-          ds[e] = pe * (dpe - (e ? dl.y : dl.x)) * sc;
-        }
-        pfrag[j >> 1][(j & 1) * 2 + i] = pack_h2<kBf16>(p[0], p[1]);
-        const uint32_t dsp = pack_h2<kBf16>(ds[0], ds[1]);
-        dsfrag[j >> 1][(j & 1) * 2 + i] = dsp;
-        if constexpr (kDQ) {
-          // dS^T -> smem row (key) of chunk j / 8, 128B-swizzled: 16-byte unit u of row r lives at unit (u ^ (r & 7))
-          const uint32_t r = (uint32_t)(kr + 8 * i), u = (uint32_t)j & 7u;
-          asm volatile("st.shared.b32 [%0], %1;" ::"r"(sDS + (j >> 3) * 16384 + r * 128u + ((u ^ (r & 7u)) << 4) +
-                                                          4u * quad),
-                       "r"(dsp)
-                       : "memory");
         }
       }
-    }
+    };
+    if (interior && args.alibi == nullptr) softmax_bwd(std::false_type{});
+    else softmax_bwd(std::true_type{});
     if constexpr (kDQ) {
       fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
       // the reduce-add issued two tiles ago has read the staging buffer this tile writes (ordered by the barrier)
       if (tid == 0) tma_store_wait_read<1>();
     }
+    mark(it, 5);
     mma_sync();
+    mark(it, 6);
     // ---- (e) dQ = dS K, then (c) dV += P^T dO, (d) dK += dS^T Q: dQ is its own group, so the dQ tile is staged and
     // reduced while the tensor cores work on dV / dK ----
     float dq[kDQ ? 32 : 1];
@@ -291,6 +362,7 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
     for (int kk = 0; kk < kQTile / 16; ++kk)
       wgmma_rs<D, kBf16, 1>(dk, dsfrag[kk], desc_mnmajor_sw128(q_s, kk, kQChunk), (it | kk) != 0);
     wgmma_commit();
+    mark(it, 7);
     if constexpr (kDQ) {
       wgmma_wait<1>();
       wgmma_fence_acc(dq);
@@ -316,11 +388,16 @@ flash_bwd_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         tma_reduce_add_3d(&tmap_dq, stg + 8192, dq_col0 + 32, h, row);
         tma_store_commit();
       }
+      mark(it, 8);
     }
     wgmma_wait<0>();
     wgmma_fence_acc(dv);
     wgmma_fence_acc(dk);
+    mark(it, 9);
     if (tid == 0) mbar_arrive(qdo_empty(s));
+  }
+  if constexpr (kProf) {
+    if (prof != nullptr && tid == 0) prof[4 + wg] = prof_clock();
   }
   if constexpr (kDQ) {
     if (tid == 0) tma_store_wait<0>();   // staging buffers stay allocated until the reduce-adds have completed
@@ -623,12 +700,12 @@ static CUtensorMap make_map_dq_acc(float* acc, long long tokens, int heads, int 
   return make_tensor_map(acc, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
-template <int D, bool kBf16, bool kDrop, bool kDQ>
+template <int D, bool kBf16, bool kDrop, bool kDQ, bool kProf = false>
 static cudaError_t launch_bwd(const CUtensorMap& mq, const CUtensorMap& mk, const CUtensorMap& mv,
                               const CUtensorMap& mdo, const CUtensorMap& mdq, const BwdArgs& a, int num_k_tiles,
                               cudaStream_t stream) {
   using S = BwdSmem<D, kDrop>;
-  auto kern = flash_bwd_kernel<D, kBf16, kDrop, kDQ>;
+  auto kern = flash_bwd_kernel<D, kBf16, kDrop, kDQ, kProf>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal);
@@ -654,6 +731,16 @@ static cudaError_t launch_bwd_dq(const CUtensorMap& mq, const CUtensorMap& mk, c
   dim3 grid(a.num_q_tiles, a.Hq, a.B);
   kern<<<grid, kBwdThreads, S::kTotal, stream>>>(mq, mk, mv, mdo, a);
   return cudaGetLastError();
+}
+
+// phase-profile buffer of the next main-kernel launches (attn_bwd_set_profile), null: profiling off
+static unsigned long long* g_prof = nullptr;
+static long long g_prof_ctas = 0;
+
+long long attn_bwd_set_profile(unsigned long long* buf, long long ctas) {
+  g_prof = buf;
+  g_prof_ctas = buf != nullptr ? ctas : 0;
+  return kProfCtaWords;
 }
 
 cudaError_t flash_attn_bwd(const AttnParams& p, int num_sms, cudaStream_t stream) {
@@ -696,12 +783,16 @@ cudaError_t flash_attn_bwd(const AttnParams& p, int num_sms, cudaStream_t stream
   a.lse = p.lse; a.delta = p.delta;
   a.dk = (uint16_t*)p.dk; a.dv = (uint16_t*)p.dv;
   a.dk_ts = p.dk_ts; a.dv_ts = p.dv_ts;
+  a.prof = g_prof; a.prof_ctas = g_prof_ctas;
   const int max_k = p.cu_k ? (int)p.Tk : p.Sk;
   const int num_k_tiles = (max_k + kTile - 1) / kTile;
 #define TB_BWD(DD, BF, DQ)                                                                        \
   (drop ? launch_bwd<DD, BF, true, DQ>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream)         \
         : launch_bwd<DD, BF, false, DQ>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream))
-  if (!deterministic) {
+  if (g_prof != nullptr && D == 64 && is_bf16 && !drop) {   // the profiled instantiations: the flagship's only
+    e = deterministic ? launch_bwd<64, true, false, false, true>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream)
+                      : launch_bwd<64, true, false, true, true>(mq, mk, mv, mdo, mdq, a, num_k_tiles, stream);
+  } else if (!deterministic) {
     if (is_bf16) e = (D == 128) ? TB_BWD(128, true, true) : TB_BWD(64, true, true);
     else e = (D == 128) ? TB_BWD(128, false, true) : TB_BWD(64, false, true);
   } else {

@@ -126,6 +126,9 @@ TB_API int tb_flash_attn_fwd(const tb::AttnParams* p, uint64_t stream) { return 
 TB_API int tb_flash_attn_bwd(const tb::AttnParams* p, int num_sms, uint64_t stream) {
   return (int)tb::flash_attn_bwd(*p, num_sms, S(stream));
 }
+TB_API long long tb_attn_bwd_set_profile(uint64_t buf, long long ctas) {
+  return tb::attn_bwd_set_profile(P<unsigned long long>(buf), ctas);
+}
 // sizeof(AttnParams), then the offset of every field in declaration order, into out[0, n); returns the number of values
 TB_API int tb_attn_params_layout(long long* out, int n) {
   using A = tb::AttnParams;
