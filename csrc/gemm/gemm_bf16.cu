@@ -851,12 +851,47 @@ cudaError_t gemm_bf16(const void* A, const void* B, void* D, const void* bias, i
                       out_fp32, cluster, num_sms, stream, is_fp16);
 }
 
+// K == 0: the product is empty, so D = bias (+ C) with the epilogue's arithmetic (an fp32 sum starting from a zero
+// accumulator, one rounding): zeros without bias or addend, D unchanged when accumulating (C == D).  This is the weight
+// gradient of a linear layer on an empty token batch.
+template <bool kBf16>
+__global__ void __launch_bounds__(256)
+gemm_empty_k_kernel(void* D, const uint16_t* bias, const void* C, int M, int N, long long ldd, long long ldc, int out_fp32) {
+  auto ld1 = [](const uint16_t* p) {
+    return kBf16 ? __bfloat162float(*reinterpret_cast<const __nv_bfloat16*>(p))
+                 : __half2float(*reinterpret_cast<const __half*>(p));
+  };
+  const long long total = (long long)M * N;
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / N;
+    const int c = (int)(i - r * N);
+    float v = 0.f;
+    if (bias) v += ld1(bias + c);
+    if (out_fp32) {
+      if (C) v += reinterpret_cast<const float*>(C)[r * ldc + c];
+      reinterpret_cast<float*>(D)[r * ldd + c] = v;
+    } else {
+      if (C) v += ld1(reinterpret_cast<const uint16_t*>(C) + r * ldc + c);
+      reinterpret_cast<uint16_t*>(D)[r * ldd + c] = (uint16_t)(pack_h2<kBf16>(v, 0.f) & 0xffffu);
+    }
+  }
+}
+
 cudaError_t gemm_bf16_ex(const void* A, const void* B, void* D, const void* bias, const void* C, int M, int N, int K,
                          long long lda, long long ldb, long long ldd, long long ldc, bool a_mn_major, bool b_mn_major,
                          bool out_fp32, int cluster, int num_sms, cudaStream_t stream, bool is_fp16) {
   if (M <= 0 || N <= 0) return cudaSuccess;
-  if (K <= 0) return cudaErrorInvalidValue;
+  if (K < 0) return cudaErrorInvalidValue;
   if (cluster != 1 && cluster != 2) return cudaErrorInvalidValue;
+  if (K == 0) {
+    long long blocks = ((long long)M * N + 255) / 256;
+    if (blocks > (long long)num_sms * 8) blocks = (long long)num_sms * 8;
+    if (blocks < 1) blocks = 1;
+    const uint16_t* b16 = reinterpret_cast<const uint16_t*>(bias);
+    if (is_fp16) gemm_empty_k_kernel<false><<<(unsigned)blocks, 256, 0, stream>>>(D, b16, C, M, N, ldd, ldc, out_fp32);
+    else gemm_empty_k_kernel<true><<<(unsigned)blocks, 256, 0, stream>>>(D, b16, C, M, N, ldd, ldc, out_fp32);
+    return cudaGetLastError();
+  }
   CUtensorMap ta, tbm;
   try {
     ta = operand_map(A, M, K, lda, a_mn_major, kBlockM);
@@ -873,9 +908,11 @@ cudaError_t gemm_bf16_ex(const void* A, const void* B, void* D, const void* bias
   const bool carrying = args.carry.slice[0].kind != 0;
   // The staged (TMA) epilogue needs D and C 16-byte aligned with row pitches of whole 16 bytes; an fp32 addend is
   // only staged as an accumulation (C == D, TMA reduce-add).  Everything else keeps the register epilogue.
+  // Rows must also end on a 16-byte boundary: at N * esz % 16 != 0 the TMA stores of a row's last box were measured
+  // writing on to that boundary on an H100, up to 7 elements past N into the caller's pitch gap.
   const long long esz = out_fp32 ? 4 : 2;
   auto aligned = [&](const void* p, long long ld) { return reinterpret_cast<uintptr_t>(p) % 16 == 0 && (ld * esz) % 16 == 0; };
-  const bool staged = !carrying && aligned(D, ldd) &&
+  const bool staged = !carrying && (N * esz) % 16 == 0 && aligned(D, ldd) &&
                       (C == nullptr || (out_fp32 ? (C == D && ldc == ldd) : aligned(C, ldc)));
   EpiMaps maps;
   memset(&maps, 0, sizeof(maps));

@@ -27,7 +27,11 @@ def _worker(rank, world, port, fn, args, errq):
         import torch.distributed as dist
         dist.init_process_group("gloo", rank=rank, world_size=world)
         fn(rank, world, *args)
-        dist.barrier()
+        # drain every group this rank belongs to (in creation order, the same on every rank) before any socket closes:
+        # a rank that tears down while a peer still has traffic on a subgroup (TP, FSDP shard groups) can abort both
+        # processes in gloo's teardown
+        for pg in list(dist.distributed_c10d._world.pg_map):
+            dist.barrier(group=pg)
         dist.destroy_process_group()
     except Exception:
         errq.put((rank, traceback.format_exc()))
