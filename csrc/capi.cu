@@ -246,6 +246,20 @@ TB_API int tb_gemm_mxfp8(uint64_t A, uint64_t sfa, uint64_t B, uint64_t sfb, uin
   return (int)tb::gemm_mxfp8(P<void>(A), P<void>(sfa), P<void>(B), P<void>(sfb), P<void>(D), P<void>(C), M, N, K, lda, ldb,
                              ldd, ldc, out_fp32 != 0, num_sms, S(stream));
 }
+TB_API int tb_gemm_grouped_mxfp8(uint64_t A, uint64_t sfa, uint64_t B, uint64_t sfb, uint64_t D, int M, int N, int K,
+                                 int E, long long lda, long long ldb, long long ldd, int b_transposed,
+                                 uint64_t tile_expert, uint64_t num_m_tiles, int num_sms, uint64_t stream) {
+  return (int)tb::gemm_grouped_mxfp8(P<void>(A), P<void>(sfa), P<void>(B), P<void>(sfb), P<void>(D), M, N, K, E, lda,
+                                     ldb, ldd, b_transposed != 0, P<const int>(tile_expert),
+                                     P<const int>(num_m_tiles), num_sms, S(stream));
+}
+TB_API int tb_gemm_grouped_wgrad_mxfp8(uint64_t A, uint64_t sfa, uint64_t B, uint64_t sfb, uint64_t D, int M, int N,
+                                       int E, int rows, long long lda, long long ldb, long long ldd, uint64_t offsets,
+                                       int out_fp32, int accumulate, int num_sms, uint64_t stream) {
+  return (int)tb::gemm_grouped_wgrad_mxfp8(P<void>(A), P<void>(sfa), P<void>(B), P<void>(sfb), P<void>(D), M, N, E,
+                                           rows, lda, ldb, ldd, P<const int>(offsets), out_fp32 != 0, accumulate != 0,
+                                           num_sms, S(stream));
+}
 // ---- mixture of experts: grouped GEMMs (gemm/gemm_bf16.cu) and routing kernels (ops/moe.cu) --------------------
 TB_API int tb_gemm_grouped(uint64_t A, uint64_t B, uint64_t D, int M, int N, int K, int E, long long lda, long long ldb,
                            long long ldd, int b_mn_major, uint64_t tile_expert, uint64_t num_m_tiles, int num_sms,

@@ -75,5 +75,17 @@ cudaError_t rs_reduce_bf16(const void* stage, const uint32_t* counters, uint32_t
 cudaError_t gemm_mxfp8(const void* A, const void* sfa, const void* B, const void* sfb, void* D, const void* C, int M,
                        int N, int K, long long lda, long long ldb, long long ldd, long long ldc, bool out_fp32,
                        int num_sms, cudaStream_t stream);
+// Grouped MX-FP8 GEMMs over expert-sorted rows (the layout of the grouped bf16 GEMMs above); bf16 output.
+// Forward (b_transposed == false): B is [E*N][K] and N % 128 == 0.  Dgrad (true): B is [N][E*K], the transposed
+// quantisation of an [E*K][N] weight.  M % 128 == 0, K % 128 == 0.
+cudaError_t gemm_grouped_mxfp8(const void* A, const void* sfa, const void* B, const void* sfb, void* D, int M, int N,
+                               int K, int E, long long lda, long long ldb, long long ldd, bool b_transposed,
+                               const int* tile_expert, const int* num_m_tiles, int num_sms, cudaStream_t stream);
+// wgrad: D[e*M : e*M + M, N] (+)= A_e B_e^T over expert e's padded rows [offsets[e], offsets[e+1]) of A [M][rows] and
+// B [N][rows] (transposed quantisations, scales along the rows); D fp32 or bf16.  rows % 128 == 0.
+cudaError_t gemm_grouped_wgrad_mxfp8(const void* A, const void* sfa, const void* B, const void* sfb, void* D, int M,
+                                     int N, int E, int rows, long long lda, long long ldb, long long ldd,
+                                     const int* offsets, bool out_fp32, bool accumulate, int num_sms,
+                                     cudaStream_t stream);
 
 }  // namespace tb
