@@ -80,19 +80,22 @@ moe_router_fwd_kernel(const void* __restrict__ logits, float* __restrict__ weigh
   int sel[kMoeMaxTopK];
   float sum = 0.f;
   for (int j = 0; j < k; ++j) {
-    // warp argmax over the experts not yet taken; ties go to the lower expert index
+    // warp argmax over the experts not yet taken; ties go to the lower expert index.  NaN ranks above every number, as
+    // in torch.topk: a non-finite logit turns the whole row into NaN probabilities, and the row must still pick k
+    // distinct experts in [0, E) (with NaN weights) rather than the out-of-range id E that the index build drops.
     float bv = -1.f;
     int be = E;
 #pragma unroll
     for (int i = 0; i < kMoeMaxExperts / 32; ++i) {
       const int e = lane + 32 * i;
-      if (e < E && !taken[i] && p[i] > bv) { bv = p[i]; be = e; }
+      if (e < E && !taken[i] && (p[i] > bv || (isnan(p[i]) && !isnan(bv)))) { bv = p[i]; be = e; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
       const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
       const int oe = __shfl_xor_sync(0xffffffffu, be, o);
-      if (ov > bv || (ov == bv && oe < be)) { bv = ov; be = oe; }
+      const bool on = isnan(ov), bn = isnan(bv);
+      if (ov > bv || (ov == bv && oe < be) || (on && (!bn || oe < be))) { bv = ov; be = oe; }
     }
 #pragma unroll
     for (int i = 0; i < kMoeMaxExperts / 32; ++i)
@@ -194,8 +197,8 @@ moe_index_kernel(const long long* __restrict__ ids, int n, int E, int rows, int*
   const unsigned lt_mask = (1u << lane) - 1u;
   for (int base = 0; base < n; base += kIndexThreads) {
     const int i = base + tid;
-    int e = i < n ? (int)ids[i] : -1;
-    if (e >= E) e = -1;
+    const long long id = i < n ? ids[i] : -1;
+    const int e = (id >= 0 && id < E) ? (int)id : -1;   // range check in 64 bits: 2^32 + 3 is not expert 3
     const unsigned peers = __match_any_sync(0xffffffffu, e);
     for (int j = tid; j < (kIndexThreads / 32) * E; j += kIndexThreads) s_warp[j / E][j % E] = 0;
     __syncthreads();

@@ -7,6 +7,9 @@
 // Scale tensors are written in the tensor core's atom order (cutlass Sm1xxBlockScaledBasicChunk): atom (row block of
 // 128, K block of 128 elements) = 512 bytes, byte (r % 32) * 16 + ((r % 128) / 32) * 4 + (kblock % 4); atoms are stored
 // [row block][K atom].  Scale = 2^ceil(log2(amax / 448)) (no saturation), element = round-to-nearest-even e4m3.
+// Non-finite input: amax skips NaN (fmaxf), so a NaN element becomes NaN alone; an infinite amax clamps the scale byte
+// at 254, whose inverse scale is 0, so the block's finite elements become +-0 and the infinity NaN
+// (fp8.quantize_mxfp8_ref emulates both).
 //
 // The reference has no fp8 support (torchacc/config.py:27-54).
 #include <cuda_fp8.h>
@@ -129,6 +132,9 @@ cudaError_t quant_mxfp8(const void* x, long long ldx, int R, int C, void* q, lon
                         long long ldqt, void* sft, cudaStream_t stream) {
   if (R <= 0 || C <= 0) return cudaSuccess;
   if (ldx % 8 != 0 || (q && ldq % 16 != 0) || (qt && ldqt % 16 != 0)) return cudaErrorInvalidValue;
+  // the kernel loads x and stores q / qt 16 bytes at a time
+  const auto misaligned = [](const void* p) { return reinterpret_cast<uintptr_t>(p) % 16 != 0; };
+  if (misaligned(x) || (q && misaligned(q)) || (qt && misaligned(qt))) return cudaErrorInvalidValue;
   dim3 grid((C + kTile - 1) / kTile, (R + kTile - 1) / kTile);
   quant_mxfp8_kernel<<<grid, 256, 0, stream>>>((const __nv_bfloat16*)x, ldx, R, C, (uint8_t*)q, ldq, (uint8_t*)sf,
                                                (C + kTile - 1) / kTile, (uint8_t*)qt, ldqt, (uint8_t*)sft,

@@ -48,6 +48,8 @@ COUNT_CASES = {
     "mixed": [0, 1, 127, 128, 129, 300, 5, 2],
     "one_expert": [512, 0, 0, 0],
     "e128": [(i * 37) % 50 for i in range(128)],
+    "last_expert": [0] * 63 + [4096],                 # every entry to expert E - 1
+    "e256": [(i * 53) % 500 for i in range(256)],     # 62 rounds of 1024 entries, counts up to 498
 }
 
 

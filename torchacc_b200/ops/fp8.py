@@ -68,6 +68,9 @@ def quantize_mxfp8(x: torch.Tensor, rowwise: bool = True, colwise: bool = False)
     assert x.dim() == 2 and x.dtype == torch.bfloat16 and x.stride(1) == 1 and x.stride(0) % 8 == 0
     R, C = x.shape
     dev = x.device
+    if x.data_ptr() % 16 != 0:   # the kernel loads 16 bytes at a time: copy a view such as x[:, 1:] to an aligned base
+        pitch = -(-max(x.stride(0), C) // 8) * 8
+        x = torch.empty((R, pitch), dtype=x.dtype, device=dev)[:, :C].copy_(x)
     row = col = None
     q = sf = qt = sft = None
     if rowwise:
@@ -123,13 +126,20 @@ def dequantize_mxfp8(t: MXTensor) -> torch.Tensor:
 
 
 def quantize_mxfp8_ref(x: torch.Tensor) -> torch.Tensor:
-    """fp32 value of x after MX-FP8 quantisation along the last dim (pure PyTorch, any device)."""
+    """fp32 value of x after MX-FP8 quantisation along the last dim (pure PyTorch, any device), as the kernel computes
+    it, non-finite input included:
+      - a NaN element does not enter its block's amax (the kernel takes it with fmaxf): the block keeps the scale of its
+        finite elements and only the NaN element quantises to NaN;
+      - an infinite element clamps the scale to 2^127, whose inverse the kernel multiplies by is 0 in fp32: the
+        infinity quantises to NaN and every finite element of its block to +-0."""
     R, C = x.shape
     xb = x.float().reshape(R, C // BLOCK, BLOCK)
-    amax = xb.abs().amax(-1, keepdim=True)
-    e = torch.ceil(torch.log2(amax / 448.0)).clamp(min=-126)
+    a = xb.abs()
+    amax = torch.where(torch.isnan(a), torch.zeros_like(a), a).amax(-1, keepdim=True)
+    e = torch.ceil(torch.log2(amax / 448.0)).clamp(min=-126, max=127)
     scale = torch.where(amax > 0, torch.pow(2.0, e), torch.ones_like(amax))
-    q = (xb / scale).to(torch.float8_e4m3fn).float()
+    inv = torch.where(torch.isinf(amax), torch.zeros_like(amax), 1.0 / scale)
+    q = (xb * inv).to(torch.float8_e4m3fn).float()
     return (q * scale).reshape(R, C)
 
 

@@ -200,7 +200,7 @@ class MoEIndex:
     """Device-resident routing schedule of one call (see csrc/ops/moe.cu, moe_index_kernel)."""
 
     def __init__(self, expert_ids: torch.Tensor, num_experts: int):
-        ids = expert_ids.reshape(expert_ids.shape[0], -1)
+        ids = expert_ids.reshape(-1, expert_ids.shape[-1])   # [T, k]; -1 in the last place is ambiguous at T = 0
         if ids.dtype != torch.int64:
             ids = ids.long()
         ids = ids.contiguous()
